@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — SLAM+NeRF frames/sec on the synthetic 640x480 stream (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
 
 A STEP = one input frame of the procedural Replica-shaped stream (BASELINE.json configs[1]:
@@ -38,10 +38,10 @@ if ROOT not in sys.path:
 
 W_IMG, H_IMG = 640, 480
 STREAM_STEP = 0.035           # camera pace: ~every 3rd-4th frame becomes a keyframe
-NERF_SM_BUDGET_SHARED = 72    # SMs of the persistent NeRF kernels when SLAM and NeRF share one GPU (N = 1)
+NERF_SM_BUDGET_SHARED = 64    # SMs of the persistent NeRF kernels when SLAM and NeRF share one GPU (N = 1): about half
 # --workload: cfg2 = BASELINE.json configs[1] (the metric's configuration, default); cfg5 = configs[4]'s shapes
 # (1280x720, buffer 200); cfg4 = configs[3] (640x480, buffer 400, plus the global-BA / alt-corr pass over the filled
-# window, timed separately as `global_ba`).  The driver runs the default; the others are recorded under profiles/.
+# window, timed separately as `global_ba`).
 WORKLOADS = {"cfg2": dict(w=640, h=480, buffer=100, corr_slots=112, name="configs[1]: Replica-office0-shaped synthetic 640x480"),
              "cfg4": dict(w=640, h=480, buffer=400, corr_slots=112, name="configs[3]: long synthetic 640x480 trajectory, buffer=400, global BA on the alt-corr path"),
              "cfg5": dict(w=1280, h=720, buffer=200, corr_slots=64, name="configs[4]: synthetic 1280x720, buffer=200")}
@@ -55,7 +55,8 @@ def set_workload(name):
 
 
 def peaks():
-    p = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "_src": "fallback"}
+    # NVIDIA's H100 SXM data sheet (700 W part): dense BF16 989 TFLOP/s, HBM3 3.35 TB/s -- data-sheet figures, not measured
+    p = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "_src": "H100 SXM data sheet"}
     f = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(f):
         p.update(json.load(open(f)))
@@ -134,10 +135,9 @@ class SlamNerfJob:
             self.nf = NerfFusion("nerf", args, self.dev)
             self.nerf_stream = torch.cuda.Stream(priority=0) if world == 1 else torch.cuda.current_stream()
             if world == 1 and "NSLAM_NERF_SMS" not in os.environ:
-                # sharing the GPU with SLAM: the persistent NeRF kernels stay on 72 of the 148 SMs.  Unbounded, the
+                # sharing the GPU with SLAM: the persistent NeRF kernels stay on about half of the SMs.  Unbounded, the
                 # latency-critical SLAM kernels wait for NeRF CTAs to retire (persistent CTAs are not pre-empted); too
                 # small a share stretches every NeRF kernel and with it the time both streams fight for the rest of the GPU.
-                # Measured at 28 / 40 / 56 / 72 SMs: 182 / 186-192 / 197 / 202 frames/s (profiles/r02_bench_call2[12]_nerf_sms*.json)
                 self.nf.ngp.num_sms = min(self.nf.ngp.num_sms, NERF_SM_BUDGET_SHARED)
         # SLAM is the latency-critical chain (host decisions wait on it): its kernels run on a HIGH-priority
         # stream so that NeRF training on the same GPU only fills the gaps
@@ -341,6 +341,8 @@ def run_ours(a):
         clocks.start()
     ms_dev, st_dev = timed(dev_frames, e2e=False)
     clk = clocks.stop() if rank == 0 else None
+    if a.dump_outputs and rank == 0:
+        dump_outputs(job, a.dump_outputs)
     # the e2e arm starts from a fresh, re-primed state so that both arms see the same keyframe budget (buffer=100)
     job_ref[0] = None
     del dev_frames, job
@@ -407,9 +409,37 @@ def run_ours(a):
     print(json.dumps(line), flush=True)
 
 
+def dump_outputs(job, out_dir):
+    """What the timed (device-resident) arm computed by its last step, as float32 .npy files in `out_dir`: the keyframe
+    poses and inverse depths a SLAM caller receives, the last keyframe's full-resolution inverse depth, and the NeRF
+    model (MLP weights and a fixed, seeded sample of the hash-grid parameters).  The stream and all seeds are fixed, so
+    two builds run with the same arguments can be compared file by file; one build writes the same files on every
+    run.  About 10 MB at the default workload."""
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {}
+    if job.is_slam:
+        fe = job.fe
+        k = int(fe.kf_idx)
+        arrays["slam_keyframe_poses"] = fe.cam0_T_world[:k]
+        arrays["slam_keyframe_idepths"] = fe.cam0_idepths[:k]
+        arrays["slam_keyframe_idepths_cov"] = fe.cam0_idepths_cov[:k]
+        arrays["slam_last_keyframe_idepth_up"] = fe.cam0_idepths_up[max(k - 1, 0)]
+    if job.is_nerf:
+        ngp = job.nf.ngp
+        arrays["nerf_mlp_weights"] = ngp.mlp
+        g = torch.Generator().manual_seed(0)
+        n = ngp.grid_master.numel()
+        idx = torch.randint(0, n, (min(n, 1 << 20),), generator=g).to(ngp.grid_master.device)
+        arrays["nerf_grid_sample"] = ngp.grid_master[idx]
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
+
+
 def _time_kernel(torch, fn, dev, iters=8, skip=3):
     """CUDA-event timing on the launching (current) stream of ONE launch at a time, L2 flushed before each (a write
-    of 256 MB > the 126 MB L2), device idle before and after: the isolated case -> compare with the BURST peaks"""
+    of 256 MB > the 50 MB L2), device idle before and after: the isolated case -> compare with the BURST peaks"""
     flush = torch.empty(64 * 1024 * 1024, device=dev)
     ts = []
     for i in range(iters):
@@ -419,16 +449,6 @@ def _time_kernel(torch, fn, dev, iters=8, skip=3):
         if i >= skip:
             ts.append(e0.elapsed_time(e1))
     return float(np.mean(ts))
-
-
-# DRAM traffic per launch (dram__bytes_read.sum + dram__bytes_write.sum) from the committed `ncu --set full` captures,
-# keyed by kernel; None where no capture at the live size exists.  See profiles/README.md.
-NCU_TRAFFIC = {
-    "conv_zr": (93056256, "profiles/r02_ncu_raw_call12.csv (18 edges)"),
-    "conv_q": (129829120, "profiles/r02_ncu_raw_call12.csv (18 edges)"),
-    "corr_lookup": (174011648, "profiles/r02_ncu_raw_call12.csv (18 edges)"),
-    "ngp_backward": (28515840, "profiles/r02_ncu_raw_call12.csv (2^18 samples)"),
-}
 
 
 def kernel_shares(job, st):
@@ -469,7 +489,7 @@ def kernel_shares(job, st):
     counts = {"total": int(up[1] * st["updates"] + fr[1] * st["frames"] + ne[1] * st["nerf_iters"]),
               "own_per_update_call": up[1], "all_per_update_call": up[2], "own_per_frame_front": fr[1],
               "all_per_frame_front": fr[2], "own_per_nerf_iter": ne[1], "all_per_nerf_iter": ne[2],
-              "note": "own = kernels of libnslam_sm100a.so; the remainder are torch glue (index/copy/normalise) kernels; "
+              "note": "own = kernels of libnslam_sm90a.so; the remainder are torch glue (index/copy/normalise) kernels; "
                       "per-keyframe extras (context encoder, correlation volumes of new edges) are not included in total"}
     shares = [{"kernel": k[:110], "share": round(v / total_us, 4)} for k, v in top]
     return shares, counts
@@ -485,23 +505,20 @@ def roofline_entries(job, pk):
     fe, dev = job.fe, job.dev
     E, hw = int(fe.ii.shape[0]), fe.ht * fe.wd
     tf_peak, hbm_peak = pk["bf16_tflops"], pk["hbm_gbs"]
-    NCU = NCU_TRAFFIC if WL is WORKLOADS["cfg2"] else {}          # the committed captures are of the 640x480 workload
     src = pk["_src"] + " (burst figures: each kernel is timed alone, device idle around it)"
     out = {}
 
     def tensor_entry(key, name, flops, ms, extra=None):
         e = {"kernel": name, "bound": "tensor", "achieved": round(flops / ms / 1e9, 1), "peak": tf_peak, "unit": "TFLOP/s",
              "frac": round(flops / ms / 1e9 / tf_peak, 3), "launch_ms": round(ms, 4), "edges": E,
-             "algorithmic_flops_per_launch": flops, "peak_source": src,
-             "traffic": NCU.get(key, (None, None))[0], "traffic_source": NCU.get(key, (None, None))[1]}
+             "algorithmic_flops_per_launch": flops, "peak_source": src}
         e.update(extra or {})
         out[key] = e
 
     def hbm_entry(key, name, nbytes, ms, edges, extra=None):
         e = {"kernel": name, "bound": "hbm", "achieved": round(nbytes / ms / 1e6, 1), "peak": hbm_peak, "unit": "GB/s",
              "frac": round(nbytes / ms / 1e6 / hbm_peak, 3), "launch_ms": round(ms, 4), "edges": edges,
-             "algorithmic_bytes_per_launch": nbytes, "peak_source": src,
-             "traffic": NCU.get(key, (None, None))[0], "traffic_source": NCU.get(key, (None, None))[1]}
+             "algorithmic_bytes_per_launch": nbytes, "peak_source": src}
         e.update(extra or {})
         out[key] = e
     op = fe.update_tc
@@ -523,7 +540,7 @@ def roofline_entries(job, pk):
     st = fe._static
     if st is not None and st.op_ctx is not None:
         ms = _time_kernel(torch, lambda: op.step(st.op_ctx), dev)
-        tensor_entry("update_operator", "nslam_update_op_step (A5: all 15 tcgen05 implicit-GEMM convolutions + glue of UpdateModule.forward)",
+        tensor_entry("update_operator", "nslam_update_op_step (A5: all 15 wgmma implicit-GEMM convolutions + glue of UpdateModule.forward)",
                      2.0 * 2283008 * hw * E, ms, {"note": "2*2,283,008 MAC per edge-pixel (SURVEY.md §8a A5); includes the glue kernels' time"})
     # HBM-bound correlation kernels
     coords1, _ = fe.reproject(fe.ii, fe.jj)
@@ -574,7 +591,7 @@ def roofline_entries(job, pk):
                                                      ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), "backward_tc")
             ms = _time_kernel(torch, bwd, dev)
             ms_step = _time_kernel(torch, tb.train_step, dev)
-        tensor_entry("ngp_backward", "ngp::backward_tc_kernel (+ grid scatter) (B3: MLP backward on tcgen05, recompute + dW + dX)",
+        tensor_entry("ngp_backward", "ngp::backward_tc_kernel (+ grid scatter) (B3: MLP backward on wgmma, recompute + dW + dX)",
                      3.0 * 2 * 10240 * n, ms, {"samples": n, "num_sms": tb.num_sms, "edges": None,
                                                "note": "3 x forward MACs (recompute, dW, dX) x samples of one batch"})
         out["ngp_backward"]["train_step_ms"] = round(ms_step, 4)
@@ -717,6 +734,8 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference", "reference-cuda"])
     ap.add_argument("--nerf-iters", type=int, default=2)
     ap.add_argument("--workload", default="cfg2", choices=sorted(WORKLOADS))
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed path computed in its last step as DIR/<name>.npy (float32)")
     a = ap.parse_args()
     set_workload(a.workload)
     if a.impl == "reference":

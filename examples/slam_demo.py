@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""The reference's entry point (examples/slam_demo.py) on the sm_100a implementation: same command line, e.g.
+"""The reference's entry point (examples/slam_demo.py) on the sm_90a implementation: same command line, e.g.
 
   python examples/slam_demo.py --dataset_dir=DIR --dataset_name=nerf --buffer=100 --slam --fusion=nerf [--eval]
   python examples/slam_demo.py --dataset_dir=synthetic --dataset_name=nerf --buffer=100 --slam --fusion=nerf

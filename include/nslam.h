@@ -1,4 +1,4 @@
-/* C ABI of libnslam_sm100a.so — hand-written sm_100a kernels behind the reference's
+/* C ABI of libnslam_sm90a.so — hand-written sm_90a kernels behind the reference's
  * `droid_backends` operator surface (reference src/droid.cpp:347-363) and the Python-side hot
  * loops around it.  Every entry point takes raw DEVICE pointers, sizes and a cudaStream_t
  * (as void*), launches on that stream, never synchronises the host and returns 0 or a
@@ -34,7 +34,7 @@ int nslam_corr_lookup_pyramid(const void* const* volumes, const int* h2s, const 
                               int coords_nhwc, void* stream);
 
 /* CorrBlock.__init__ + CorrBlock.corr (networks/modules/corr.py:23-38,63-72): all-pairs
- * correlation (f1/4).(f2/4) and the 3 avg-pooled levels, fp16, in one tcgen05 kernel.
+ * correlation (f1/4).(f2/4) and the 3 avg-pooled levels, fp16, in one tensor-core kernel.
  * fmaps [NF,H,W,C=128] fp16 channels-last; ii/jj [E] int32 DEVICE frame indices;
  * out_l [E,H,W,H>>l,W>>l] fp16. */
 int nslam_corr_volume_build(const void* fmaps, int NF, int H, int W, int C, const int* ii,

@@ -90,16 +90,16 @@ int nslam_ngp_ingest_batch(const unsigned char* rgb_chw, const float* idepth_up,
 int nslam_ngp_cam_grad(const void* grid_half, const float* scale16, const int* res16, const unsigned* size16,
                        const unsigned* offset16, const int* dense16, float aabb_scale, const float* rays, int max_rays,
                        const float* coords, const float* tdist, const void* denc, float loss_scale, float* cam_grad,
-                       void* stream);
+                       int n_images, void* stream);
 int nslam_ngp_cam_adam_apply(const void* base_cams, void* eff_cams, float* offsets, float* cam_grad, float* m, float* v,
                              int* steps, int n, float lr, float beta1, float beta2, float eps, float l2, void* stream);
 
-/* tensor-core (tcgen05) variants of the network forward / backward, fused with the hash encoding
- * (csrc/ngp_tc.cu).  `packed` = 61 440-byte buffer of fp16 UMMA-ready weight images (forward images
+/* tensor-core (wgmma) variants of the network forward / backward, fused with the hash encoding
+ * (csrc/ngp_tc.cu).  `packed` = 61 440-byte buffer of fp16 wgmma-ready weight images (forward images
  * B[n][k] at 0, backward images B[k][n] at 28 672) produced by nslam_ngp_pack_mlp from the fp32 MLP blob
  * (re-run after every optimiser step).  n < 0: sample count read from counters[0].  The backward
  * carries its deltas in fp16 multiplied by `loss_scale` (instant-ngp's mixed-precision recipe) and
- * accumulates weight gradients in TMEM across all tiles of a CTA. */
+ * accumulates weight gradients in registers across all tiles of a CTA. */
 int nslam_ngp_pack_mlp(const float* mlp, void* packed, void* stream);
 int nslam_ngp_forward_tc(const nslam_ngp_model* m, const void* packed, const float* coords, const int* counters,
                          int n, int max_samples, float* rgbsigma, void* enc_out, int num_sms, void* stream);

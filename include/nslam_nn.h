@@ -13,20 +13,23 @@ extern "C" {
  * (src_channels: HOST ints, each a multiple of 8); wpacked: DEVICE, packed by
  * nerf_slam_b200/conv.py::pack_weights; bias/gctx/gsum fp32 DEVICE; out0/out1 NHWC fp16 DEVICE
  * (out0 may be a channel slice: pass the pointer to its first channel and the FULL channel count
- * of the underlying tensor as out0_channels).  N in {16,64,128,256}. */
+ * of the underlying tensor as out0_channels).  N in {16,64,128,256}.
+ * partials: DEVICE fp32 scratch of B * T * 4 * N floats (T = ceil(H/8) * ceil(W/16) tiles per image) for mode 3,
+ * NULL otherwise: per-tile column sums, reduced in a fixed order into gsum (+=) so that gsum is the same on every run. */
 int nslam_conv_igemm(const void* const* srcs, const int* src_channels, int n_src, int B, int H, int W,
                      int KH, int KW, int pad, int N, const void* wpacked, const float* bias, int mode,
                      int act, const float* gctx, const void* net, const void* zbuf, float* gsum,
-                     void* out0, int out0_channels, void* out1, int num_sms, void* stream);
+                     void* out0, int out0_channels, void* out1, float* partials, int num_sms, void* stream);
 
 /* extended form: mode 4 = encoder layer (BasicEncoder, networks/modules/extractor.py:118-198):
  *   stats [B][N][2] fp32 (zeroed by the caller) or NULL: per-image channel sum / sum of squares of the fp16
- *   outputs, consumed by nslam_inorm_apply; sub = 2: stride-2 convolution (out0 is [B,ceil(H/2),ceil(W/2),C]). */
+ *   outputs, consumed by nslam_inorm_apply; sub = 2: stride-2 convolution (out0 is [B,ceil(H/2),ceil(W/2),C]).
+ *   With stats, partials = B * T * 4 * N * 2 floats of scratch (T as above, from the stride-1 H, W). */
 int nslam_conv_igemm_ex(const void* const* srcs, const int* src_channels, int n_src, int B, int H, int W,
                         int KH, int KW, int pad, int N, const void* wpacked, const float* bias, int mode,
                         int act, const float* gctx, const void* net, const void* zbuf, float* gsum,
-                        void* out0, int out0_channels, void* out1, float* stats, int sub, int num_sms,
-                        void* stream);
+                        void* out0, int out0_channels, void* out1, float* stats, int sub, float* partials,
+                        int num_sms, void* stream);
 /* im2col of the encoders' 7x7 / stride-2 / 3-channel first layer: x [B,3,H,W] fp32 -> [B,H/2,W/2,152] fp16,
  * K index = (ky*7 + kx)*3 + c (147 real columns) -> the layer runs as a 1x1 GEMM (extractor.py:139). */
 int nslam_im2col7_s2(const float* x, void* out, int B, int H, int W, void* stream);
@@ -73,6 +76,7 @@ typedef struct nslam_update_ctx {
   const void* wp[NSLAM_W_COUNT]; const float* bias[NSLAM_W_COUNT];
   const float* glo_w; const float* glo_b;                        /* [384,128], [384] fp32 */
   /* workspace (fp16 unless noted) */
+  /* gsum: [E][128] followed by the glo convolution's partials [E][T][4][128] (T = ceil(H/8) * ceil(W/16)) */
   void* c1; void* c2; void* mcol; void* f1; void* f2; float* gsum; float* gzr; float* gq;
   void* z; void* rnet; void* h0; void* h2; void* a1; void* am; void* a2; void* e16;
 } nslam_update_ctx;

@@ -1,4 +1,4 @@
-"""ctypes binding of libnslam_sm100a.so — the only way the Python host code reaches the kernels.
+"""ctypes binding of libnslam_sm90a.so — the only way the Python host code reaches the kernels.
 
 There is deliberately no fallback: if the shared object is missing or a CUDA device is absent
 the operators raise (`NslamUnavailable`), they never route through PyTorch/CPU code.
@@ -7,7 +7,7 @@ import ctypes
 import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(HERE, "libnslam_sm100a.so")
+LIB_PATH = os.path.join(HERE, "libnslam_sm90a.so")
 
 c_void_p, c_int, c_float = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
 
@@ -69,7 +69,7 @@ _SIGNATURES = {
     "nslam_segment_mean": [_P, _P, _P, _P, c_int, c_int, _P],
     "nslam_eta_damping": [_P, _P, _P, c_int, _P, _P, c_int, c_int, c_float, _P],
     "nslam_conv_igemm_ex": [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int,
-                            _P, _P, _P, _P, _P, c_int, _P, _P, c_int, c_int, _P],
+                            _P, _P, _P, _P, _P, c_int, _P, _P, c_int, _P, c_int, _P],
     "nslam_im2col7_s2": [_P, _P, c_int, c_int, c_int, _P],
     "nslam_update_op_step": [ctypes.POINTER(UpdateCtx), _P],
     "nslam_inorm_stats": [_P, _P, c_int, c_int, c_int, c_int, _P],
@@ -104,7 +104,7 @@ _SIGNATURES = {
     "nslam_ngp_ingest_image": [_P, _P, _P, c_int, c_int, _P, _P, _P, _P],
     "nslam_ngp_ingest_batch": [_P, _P, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P, c_float, c_float, c_float, c_float, _P, _P,
                                _P, _P, c_int, _P],
-    "nslam_ngp_cam_grad": [_P, _P, _P, _P, _P, _P, c_float, _P, c_int, _P, _P, _P, c_float, _P, _P],
+    "nslam_ngp_cam_grad": [_P, _P, _P, _P, _P, _P, c_float, _P, c_int, _P, _P, _P, c_float, _P, c_int, _P],
     "nslam_ngp_cam_adam_apply": [_P, _P, _P, _P, _P, _P, _P, c_int, c_float, c_float, c_float, c_float, c_float, _P],
     "nslam_ngp_pack_mlp": [_P, _P, _P],
     "nslam_ngp_forward_tc": [_P, _P, _P, _P, c_int, c_int, _P, _P, c_int, _P],
@@ -115,7 +115,7 @@ _SIGNATURES = {
     "nslam_ngp_loss_phase": [_P, c_int, c_float, c_float, c_float, c_float, _P],
     # tensor-core convolution (include/nslam_nn.h)
     "nslam_conv_igemm": [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int,
-                         _P, _P, _P, _P, _P, c_int, _P, c_int, _P],
+                         _P, _P, _P, _P, _P, c_int, _P, _P, c_int, _P],
 }
 
 _lib = None
@@ -143,7 +143,7 @@ def load(require_cuda=True):
     if require_cuda and not _cuda_ok:
         import torch
         if not torch.cuda.is_available():
-            raise NslamUnavailable("nerf_slam_b200 operators need a CUDA device (sm_100a); "
+            raise NslamUnavailable("nerf_slam_b200 operators need a CUDA device (sm_90a); "
                                    "there is no CPU fallback")
         _cuda_ok = True          # checked once: the query costs ~4 us and every operator comes through here
     return _lib

@@ -1,4 +1,4 @@
-"""Build libnslam_sm100a.so (the C-ABI library with every hand-written sm_100a kernel) in-tree.
+"""Build libnslam_sm90a.so (the C-ABI library with every hand-written sm_90a kernel) in-tree.
 
     python -m nerf_slam_b200.build [--force]
 
@@ -13,10 +13,10 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "_build")
-LIB = os.path.join(HERE, "libnslam_sm100a.so")
+LIB = os.path.join(HERE, "libnslam_sm90a.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 # NB: no --use_fast_math: frame_distance / corr lookup reproduce the reference's IEEE arithmetic.
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xptxas", "-v",
          "--expt-relaxed-constexpr", "-diag-suppress", "550"]

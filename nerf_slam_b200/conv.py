@@ -1,4 +1,4 @@
-"""Tensor-core (tcgen05) execution of the update operator — host side.
+"""Tensor-core (wgmma) execution of the update operator — host side.
 
 `UpdateOperatorTC` evaluates the reference's UpdateModule.forward (networks/droid_net.py:118-150;
 ConvGRU networks/modules/gru.py:19-32; GraphAgg networks/droid_net.py:59-75) with every 3x3 / 1x1
@@ -51,16 +51,25 @@ def pack_weights(w, src_channels, n_pad=None):
     return torch.cat(blocks).half().contiguous()
 
 
+def conv_partials(B, H, W, N, k, device):
+    """scratch of the per-tile column sums (mode 3: k = 1; mode 4 statistics: k = 2) that the kernel reduces in a
+    fixed order, 4 row quarters per 8x16-pixel tile (include/nslam_nn.h)"""
+    T = ((H + 7) // 8) * ((W + 15) // 16)
+    return torch.empty(B * T * 4 * N * k, dtype=torch.float32, device=device)
+
+
 def conv_tc(srcs, wpacked, bias, B, H, W, KH, pad, N, mode=0, act=0, gctx=None, net=None, zbuf=None,
-            gsum=None, out0=None, out0_channels=None, out1=None, num_sms=148):
+            gsum=None, out0=None, out0_channels=None, out1=None, num_sms=132):
     lib = _lib.load()
+    part = conv_partials(B, H, W, N, 1, srcs[0].device) if mode == 3 else None
     n = len(srcs)
     ptrs = (ctypes.c_void_p * n)(*[s.data_ptr() for s in srcs])
     chans = (ctypes.c_int * n)(*[s.shape[-1] for s in srcs])
     _lib.check(lib.nslam_conv_igemm(ctypes.cast(ptrs, ctypes.c_void_p), ctypes.cast(chans, ctypes.c_void_p), n,
                                     B, H, W, KH, KH, pad, N, _lib.ptr(wpacked), _lib.ptr(bias), mode, act,
                                     _lib.ptr(gctx), _lib.ptr(net), _lib.ptr(zbuf), _lib.ptr(gsum), _lib.ptr(out0),
-                                    int(out0_channels or 0), _lib.ptr(out1), num_sms, _lib.stream_ptr()), "conv_igemm")
+                                    int(out0_channels or 0), _lib.ptr(out1), _lib.ptr(part), num_sms, _lib.stream_ptr()),
+               "conv_igemm")
 
 
 def _sm_budget(device, env):
@@ -200,8 +209,9 @@ class UpdateOperatorTC:
             ctx.wp[i] = wp.data_ptr(); ctx.bias[i] = b.data_ptr() if b is not None else None
         ctx.glo_w, ctx.glo_b = self.glo_w.data_ptr(), self.glo_b.data_ptr()
         hw = H * W
+        tiles = ((H + 7) // 8) * ((W + 15) // 16)               # gsum is followed by the glo convolution's partials
         sizes = dict(c1=E * hw * 128 * 2, c2=E * hw * 128 * 2, mcol=E * hw * MOTION_COLS * 2, f1=E * hw * 128 * 2,
-                     f2=E * hw * 64 * 2, gsum=E * 128 * 4, gzr=E * 256 * 4, gq=E * 128 * 4, z=E * hw * 128 * 2,
+                     f2=E * hw * 64 * 2, gsum=E * 128 * 4 * (1 + 4 * tiles), gzr=E * 256 * 4, gq=E * 128 * 4, z=E * hw * 128 * 2,
                      rnet=E * hw * 128 * 2, h0=E * hw * 256 * 2, h2=E * hw * 16 * 2, a1=E * hw * 128 * 2,
                      am=max(K, 1) * hw * 128 * 2, a2=max(K, 1) * hw * 128 * 2, e16=max(K, 1) * hw * 16 * 2)
         total = sum((v + 255) // 256 * 256 for v in sizes.values())
@@ -242,17 +252,18 @@ class UpdateOperatorTC:
         return out[0], delta, out[2], eta, out[4]
 
 
-def conv_enc(srcs, wpacked, bias, B, H, W, k, N, out, act=0, stats=None, sub=1, num_sms=148):
+def conv_enc(srcs, wpacked, bias, B, H, W, k, N, out, act=0, stats=None, sub=1, num_sms=132):
     """encoder layer on the tensor-core kernel (mode 4): NHWC fp16 in/out, optional channel statistics for the
     instance norm that follows, optional stride 2 (out is then [B,ceil(H/2),ceil(W/2),N])"""
     lib = _lib.load()
     n = len(srcs)
     ptrs = (ctypes.c_void_p * n)(*[s.data_ptr() for s in srcs])
     chans = (ctypes.c_int * n)(*[s.shape[-1] for s in srcs])
+    part = conv_partials(B, H, W, N, 2, out.device) if stats is not None else None
     _lib.check(lib.nslam_conv_igemm_ex(ctypes.cast(ptrs, ctypes.c_void_p), ctypes.cast(chans, ctypes.c_void_p), n,
                                        B, H, W, k, k, k // 2, N, _lib.ptr(wpacked), _lib.ptr(bias), 4, act,
                                        None, None, None, None, _lib.ptr(out), out.shape[-1], None, _lib.ptr(stats), sub,
-                                       num_sms, _lib.stream_ptr()), "conv_igemm_ex")
+                                       _lib.ptr(part), num_sms, _lib.stream_ptr()), "conv_igemm_ex")
 
 
 class EncoderTC:

@@ -3,7 +3,7 @@
   CorrBlock(fmap1, fmap2, num_levels=4, radius=3)  .__call__(coords) .cat(other) .__getitem__(mask)
   AltCorrBlock(fmaps, num_levels=4, radius=3)      .__call__(coords, ii, jj)
 
-backed by the sm_100a kernels (tcgen05 volume build with fused pyramid, fused 4-level lookup,
+backed by the sm_90a kernels (wgmma volume build with fused pyramid, fused 4-level lookup,
 on-the-fly alt-corr).  `CorrPool` is the arena the front-end uses instead of `CorrBlock.cat`:
 pre-allocated pyramid slots, so adding/removing edges never re-copies volumes
 (the reference's `torch.cat` re-copies the whole pool on every add, corr.py:52-55).

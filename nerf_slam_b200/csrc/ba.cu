@@ -5,7 +5,7 @@
 // x3 (CPU argsort + CSR) -> host O(P^2 deg^2) enumeration -> EEt6x6/Ev6x1 (one CTA per
 // (i,j,k) triple, each re-reading 13*HW floats) -> Eigen dense -> GPU; then gtsam on the CPU.
 //
-// B200 design:
+// Design:
 //  * work is organised by DEPTH MAP (source frame) x PIXEL TILE, grid = (T, K): everything that
 //    the Schur complement needs for depth map k (C, w, Ei and every Ej row that shares k) is
 //    produced by the same CTA, so E is written once and read once more (L2-hot);
@@ -25,7 +25,7 @@
 
 namespace nslam {
 
-constexpr int TILE = 128;  // pixels per CTA tile (one pixel per thread); 640x480/8: 38 tiles x K maps fills the 148 SMs twice
+constexpr int TILE = 128;  // pixels per CTA tile (one pixel per thread); 640x480/8: 38 tiles x K maps keeps all SMs busy
 constexpr int AUX = 80;    // floats per edge in edge_aux
 
 // ------------------------------------------------------------------------------------------

@@ -1,4 +1,4 @@
-// Shared device helpers for the nerf_slam_b200 kernels (sm_100a).
+// Shared device helpers for the nerf_slam_b200 kernels (sm_90a).
 //
 // Conventions (same as the reference's droid_backends, src/droid_kernels.cu):
 //   pose      = [tx ty tz qx qy qz qw]  (camera-from-world, Hamilton quaternion, w last)

@@ -1,5 +1,5 @@
-// Shared pieces of the implicit-GEMM convolution kernels (conv_igemm.cu: one CTA per tile;
-// conv_igemm2.cu: CTA pairs, cta_group::2): launch parameters, shared-memory plan, epilogue math.
+// Shared pieces of the implicit-GEMM convolution kernel (conv_igemm.cu): launch parameters, shared-memory plan,
+// epilogue math.
 #pragma once
 #include <atomic>
 #include "common.cuh"
@@ -7,14 +7,12 @@
 
 namespace nslam {
 
-constexpr int CG_EPI_WARPS = 8;
-constexpr int CG_THREADS_BASE = 64 + 32 * CG_EPI_WARPS;     // TMA warp, MMA warp, 8 epilogue warps (conv_halo.cu, conv_igemm2.cu)
-// conv_igemm.cu adds three more TMA-issuing warps behind the epilogue warps.  One warp issues a cp.async.bulk every ~280
-// cycles and a tensor-map load every ~500-630, whatever their size — but different warps of an SM overlap
-// (tools/probes/umma_rate_probe.cu, profiles/r02_tma_multi_warp_probe_call9.log): with a single producer warp a 64-channel
-// block of a 3x3 convolution (3 boxes + 9 weight blocks) cost ~5200 cycles of issue against 2304 cycles of MMAs at N = 128.
-constexpr int CG_A_WARPS = 2, CG_W_WARPS = 2;              // activation-box issuers: warps 0 and 10; weight issuers: 11, 12
-constexpr int CG_THREADS = CG_THREADS_BASE + 32 * (CG_A_WARPS - 1 + CG_W_WARPS);
+constexpr int CG_EPI_WARPS = 8;                            // two warpgroups: MMA + epilogue
+// Four TMA-issuing warps (one warpgroup) behind them: a single warp issues one cp.async.bulk / tensor-map load at a
+// time, different warps of an SM overlap, and a 64-channel block of a 3x3 convolution is 3 boxes + 9 weight blocks.
+constexpr int CG_A_WARPS = 2, CG_W_WARPS = 2;              // activation-box issuers: warps 8, 9; weight issuers: 10, 11
+constexpr int CG_THREADS = 32 * (CG_EPI_WARPS + CG_A_WARPS + CG_W_WARPS);
+constexpr int CG_SCR_LD = 40;                              // fp32 accumulator chunk per warpgroup: [128][32 + 8 padding]
 template <int N> struct CgStages { static constexpr int value = (N >= 256) ? 3 : 4; };
 constexpr int CG_TH = 8, CG_TW = 16;
 
@@ -35,6 +33,7 @@ struct ConvParams {
   float* gsum;             // [B][128] (mode 3)
   float* stats;            // [B][N][2] per-image channel sum / sum of squares of the fp16 outputs (mode 4) or null
   int sub;                 // mode 4: 1 = store every pixel, 2 = store (and count) even rows/cols only (stride-2 conv)
+  float* partials;         // modes 3 / 4 with stats: per-(tile, row quarter) column sums [B*T][4][N][1 or 2]
 };
 
 struct ConvMaps {
@@ -76,16 +75,18 @@ struct CgSmem {
   static constexpr int A_STAGE = HALO ? 20480 : 16384;
   // the loops are latency-bound on the weight blocks (one 1-D bulk copy per tap and channel block, ~1.5 us
   // round trip): keep as many of them in flight as shared memory allows
-  static constexpr int A_STAGES = HALO ? 3 : STAGES;
-  static constexpr int B_STAGES = HALO ? ((N >= 256) ? 4 : 8) : STAGES;
+  static constexpr int A_STAGES = HALO ? ((N >= 256) ? 2 : 3) : STAGES;
+  static constexpr int B_STAGES = HALO ? ((N >= 256) ? 3 : (N >= 128 ? 4 : 8)) : STAGES;
   static constexpr int A = 0;
   static constexpr int B = A_STAGES * A_STAGE;
   static constexpr int OUT = B + B_STAGES * N * 128;
   static constexpr int PASSES = (N >= 256) ? 2 : 1;        // N = 256: the epilogue stages / stores 128 columns at a time
   static constexpr int NOUT64 = (N >= 64) ? (N / PASSES) / 64 : 1;    // 64-channel staging tiles
   static constexpr int BIAS = OUT + NOUT64 * 16384;
-  static constexpr int BAR = BIAS + 3 * N * 4;     // bias | column sums | column sums of squares
+  static constexpr int SCR = BIAS + N * 4;         // bias
+  static constexpr int BAR = SCR + 2 * 128 * CG_SCR_LD * 4;
   static constexpr int TOTAL = BAR + 256;
+  static_assert(TOTAL + 1024 <= 227 * 1024, "shared memory plan");
 };
 
 // transpose-reduce: on entry lane l holds v[0..31] (32 columns of ITS pixel); on exit every lane
@@ -153,14 +154,5 @@ __device__ __forceinline__ void epi_chunk(const uint32_t (&r)[32], float (&v)[32
     }
   }
 }
-
-// second generation for 3x3 / pad 1 (conv_halo.cu): 16x16 super-tiles, one halo box per channel block
-bool conv_halo_supported(int N, int mode, int KH, int KW, int pad);
-int launch_conv_halo(int N, const ConvMaps& maps, const ConvParams& p, int num_sms, cudaStream_t st);
-
-// CTA-pair variant (conv_igemm2.cu), opt-in: NSLAM_CONV_CTA2=1
-bool conv_pairs_enabled();
-bool conv_pairs_supported(int N, int mode, bool halo);
-int launch_conv_pairs(int N, const ConvMaps& maps, const ConvParams& p, int num_sms, cudaStream_t st);
 
 }  // namespace nslam

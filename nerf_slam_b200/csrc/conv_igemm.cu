@@ -1,4 +1,4 @@
-// A5/A1 — convolutions of the update operator as implicit GEMM on tcgen05 (sm_100a).
+// A5/A1 — convolutions of the update operator as implicit GEMM on Hopper tensor cores (wgmma, sm_90a).
 //
 // Replaces the cuDNN convolutions behind UpdateModule / ConvGRU / GraphAgg
 // (reference networks/droid_net.py:78-150, networks/modules/gru.py:5-32) and the
@@ -13,12 +13,13 @@
 //   (dy,dx) the A tile is the TMA box {64c, 16w, 8h} shifted by (dx-pad, dy-pad): out-of-image
 //   rows/cols are zero-filled by TMA, which IS the convolution's zero padding;
 // * weights are pre-packed on the host into the exact 128B-swizzled K-major smem image, one
-//   contiguous N*128-byte block per (tap, channel-block): a 1-D bulk copy lands it UMMA-ready;
-// * 4-stage mbarrier ring, one thread issues tcgen05.mma (M128, N, K16), fp32 accumulators in
-//   TMEM, double buffered so the epilogue of tile t overlaps the MMAs of tile t+1;
+//   contiguous N*128-byte block per (tap, channel-block): a 1-D bulk copy lands it wgmma-ready;
+// * mbarrier rings fed by a warpgroup of TMA-issuing warps; two consumer warpgroups each own half of
+//   the output columns (N >= 64) and issue wgmma (2 x M64, N/2 or N/4 per pass, K16) into fp32
+//   register accumulators;
 // * persistent CTAs (grid = #SMs) walk the (image, tile) list;
-// * epilogue (8 warps, thread = pixel, the two warps of a TMEM lane quarter split the columns):
-//   tcgen05.ld -> +bias (+ per-image global-context vector) -> activation / GRU gating -> fp16 ->
+// * epilogue (the same two warpgroups, thread = pixel): accumulators -> 32-column fp32 shared tile ->
+//   +bias (+ per-image global-context vector) -> activation / GRU gating -> fp16 ->
 //   swizzled smem -> TMA store (clips partial tiles).  Kernel templated on the epilogue mode.
 //
 // Epilogue modes:
@@ -26,18 +27,17 @@
 //   1 ZR    N = 256: z = sigmoid(acc[0:128]+..), r = sigmoid(acc[128:256]+..);
 //           out0 = z, out1 = r * net          (ConvGRU z,r gates, gru.py:27-29)
 //   2 Q     q = tanh(acc + ..); out0 = (1 - z) * net + z * q         (gru.py:29-31)
-//   3 GLO   y = sigmoid(acc + bias) * net; per-tile column sums (warp transpose-reduce -> shared
-//           accumulator) added to gsum[n][c] (fp32)  -> glo = mean (gru.py:23-25); nothing is stored
+//   3 GLO   y = sigmoid(acc + bias) * net; per-tile column sums (warp transpose-reduce, one partial per warp and
+//           tile, no atomics) reduced in a fixed order into gsum[n][c] (fp32) -> glo = mean (gru.py:23-25); nothing
+//           is stored
 //   4 ENC   encoder layers (BasicEncoder, extractor.py): y = act(acc + bias) like mode 0, plus (a) optional
 //           per-(image, channel) sum / sum of squares of the fp16 outputs for the instance norm that follows
 //           and (b) optional stride-2 output: the conv is evaluated at stride 1 and only even rows/columns
 //           are stored and counted (a 3x3/s2 conv reads every input pixel anyway).
 // Roofline: tensor pipe; FLOPs = 2 * pixels * taps * Cin * Cout.
-#include <cstdlib>
 #include "conv_common.cuh"
 
 namespace nslam {
-constexpr uint32_t CH2_BOX = 18;        // halo box edge of conv_halo.cu (16 + 2)
 
 template <int N, int MODE, bool HALO>
 __global__ void __launch_bounds__(CG_THREADS, 1)
@@ -45,8 +45,9 @@ conv_igemm_kernel(const __grid_constant__ ConvMaps maps, ConvParams p) {
   using SM = CgSmem<N, HALO>;
   constexpr int CG_STAGES = SM::STAGES;
   constexpr int AS = SM::A_STAGES, BS = SM::B_STAGES;
-  constexpr int TCOLS = (N <= 32) ? 64 : (N <= 64 ? 128 : (N <= 128 ? 256 : 512));   // 2 accumulator stages
-  constexpr int ACC_STRIDE = TCOLS / 2;
+  constexpr int PASSES = SM::PASSES, CPP = N / PASSES;          // columns staged per pass
+  constexpr int GC = (N >= 64) ? CPP / 2 : N;                   // columns per warpgroup per pass
+  constexpr int MMA_WARPS = (N >= 64) ? 8 : 4;                  // N < 64: warpgroup 0 computes every column
   extern __shared__ unsigned char smem_raw[];
   unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* bars = reinterpret_cast<uint64_t*>(sm + SM::BAR);
@@ -54,11 +55,7 @@ conv_igemm_kernel(const __grid_constant__ ConvMaps maps, ConvParams p) {
   uint64_t* empty_b = bars + BS;
   uint64_t* full_a = bars + 2 * BS;              // HALO only: the shifted-tile ring
   uint64_t* empty_a = full_a + AS;
-  uint64_t* tm_full = empty_a + AS;
-  uint64_t* tm_empty = tm_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tm_empty + 2);
   float* sbias = reinterpret_cast<float*>(sm + SM::BIAS);
-  float* sacc = sbias + N;                       // mode 3: per-CTA column sums of the current tile
   static_assert((4 * 4 + 4) * 8 + 8 <= 256, "barrier block");
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -67,28 +64,24 @@ conv_igemm_kernel(const __grid_constant__ ConvMaps maps, ConvParams p) {
   const int taps = p.KH * p.KW;
   const int nkb = taps * p.cb_total;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < p.n_src; s++) tc::tma_prefetch_desc(&maps.src[s]);
-    for (int s = 0; s < BS; s++) { tc::mbar_init(&full_b[s], HALO ? 1 : 2); tc::mbar_init(&empty_b[s], 1); }
-    for (int s = 0; s < AS; s++) { tc::mbar_init(&full_a[s], 1); tc::mbar_init(&empty_a[s], 1); }
-    for (int s = 0; s < 2; s++) { tc::mbar_init(&tm_full[s], 1); tc::mbar_init(&tm_empty[s], CG_EPI_WARPS); }
+    for (int s = 0; s < BS; s++) { tc::mbar_init(&full_b[s], HALO ? 1 : 2); tc::mbar_init(&empty_b[s], MMA_WARPS); }
+    for (int s = 0; s < AS; s++) { tc::mbar_init(&full_a[s], 1); tc::mbar_init(&empty_a[s], MMA_WARPS); }
     tc::fence_barrier_init();
   }
-  if (warp == 1) tc::tmem_alloc<TCOLS>(tmem_slot);
-  for (int i = threadIdx.x; i < N; i += CG_THREADS) { sbias[i] = p.bias ? p.bias[i] : 0.f; sacc[i] = 0.f; sacc[N + i] = 0.f; }
-  tc::tc_fence_before();
+  for (int i = threadIdx.x; i < N; i += CG_THREADS) sbias[i] = p.bias ? p.bias[i] : 0.f;
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // warp roles: 0 and 10 = activation (A) producers, 11 and 12 = weight (B) producers, 1 = MMA issuer, 2..9 = epilogue
-  const int a_part = (warp == 0) ? 0 : (warp == 2 + CG_EPI_WARPS) ? 1 : -1;
-  const int w_part = (warp >= 3 + CG_EPI_WARPS) ? warp - (3 + CG_EPI_WARPS) : -1;
+  // warp roles: 0..7 = two warpgroups (MMA + epilogue), 8 and 9 = activation (A) producers, 10 and 11 = weight (B) producers
+  const int a_part = (warp == CG_EPI_WARPS) ? 0 : (warp == CG_EPI_WARPS + 1) ? 1 : -1;
+  const int w_part = (warp >= CG_EPI_WARPS + CG_A_WARPS) ? warp - (CG_EPI_WARPS + CG_A_WARPS) : -1;
   if (a_part >= 0 || w_part >= 0) {
     // ===================== TMA producers =====================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     // Every producer warp walks the same sequence of load units and issues those of its own parity: an A warp the
     // activation loads with (counter % CG_A_WARPS) == a_part, a W warp the weight blocks with (counter % CG_W_WARPS) ==
-    // w_part.  Whole warp in the loop, elected lane issues (uniform control flow, see tc::umma_f16_lead).
+    // w_part.  Whole warp in the loop, elected lane issues (uniform control flow).
     const uint32_t lead = tc::elect_one() ? 1u : 0u;
     auto src_of = [&](int g, int& sidx, int& cb) { sidx = 0; cb = g; while (cb >= p.src_cb[sidx]) { cb -= p.src_cb[sidx]; sidx++; } };
     if (HALO) {
@@ -151,68 +144,89 @@ conv_igemm_kernel(const __grid_constant__ ConvMaps maps, ConvParams p) {
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    // The WHOLE warp runs the loop (uniform control flow: loop counters, barrier addresses and descriptors live in
-    // uniform registers); only the elected lane issues tcgen05.mma / tcgen05.commit (tc::umma_f16_lead).
-    {
-      const uint32_t lead = tc::elect_one() ? 1u : 0u;
-      constexpr uint32_t idesc = tc::umma_idesc_f16(128, N, 0);
-      uint32_t it = 0, ia = 0, tcount = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, tcount++) {
-        const int as = tcount & 1, aph = (tcount >> 1) & 1;
-        tc::mbar_wait(&tm_empty[as], aph ^ 1);
-        const uint32_t d_tmem = tmem_base + as * ACC_STRIDE;
+  } else {
+    // ===================== two warpgroups: MMA, then epilogue (thread = output pixel) =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int q = warp & 3;
+    const int grp = warp >> 2;
+    const int row = q * 32 + lane;
+    const int wtid = threadIdx.x & 127;
+    const int hh = row / CG_TW, ww = row % CG_TW;
+    const int etid = threadIdx.x;
+    const bool works = (N >= 64) || grp == 0;
+    float* scr = reinterpret_cast<float*>(sm + SM::SCR) + grp * 128 * CG_SCR_LD;
+    uint32_t it = 0, ia = 0;
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+      // ---- MMAs: this warpgroup's columns pass * CPP + grp * GC + [0, GC) of all 128 pixels
+      float acc[PASSES][2][GC / 2];
+#pragma unroll
+      for (int ps = 0; ps < PASSES; ps++)
+#pragma unroll
+        for (int hf = 0; hf < 2; hf++)
+#pragma unroll
+          for (int i = 0; i < GC / 2; i++) acc[ps][hf][i] = 0.f;
+      const uint32_t b_col = (uint32_t)((N >= 64) ? grp * GC : 0) * 128;
+      if (works) {
         if (HALO) {
           const int units = p.cb_total * 3;
           for (int u = 0; u < units; u++, ia++) {
             const int sa = ia % AS, pa = (ia / AS) & 1;
             tc::mbar_wait(&full_a[sa], pa);
-            // descriptor of the tile's first row; +dy * 16 rows (2048 B) and +k * 32 B are added in descriptor units (16 B)
-            const uint64_t a_desc = tc::umma_desc_sw128(tc::smem_u32(sm + SM::A + sa * SM::A_STAGE));
+            // the tile's first row; +dy * 16 rows (2048 B) selects the tap, +64 rows (8192 B) the second half
+            const uint32_t a_addr = tc::smem_u32(sm + SM::A + sa * SM::A_STAGE);
+            int sbs[3];
 #pragma unroll
             for (int dy = 0; dy < 3; dy++, it++) {
               const int sb = it % BS, pb = (it / BS) & 1;
+              sbs[dy] = sb;
               tc::mbar_wait(&full_b[sb], pb);
-              tc::tc_fence_after();
-              const uint64_t b_desc = tc::umma_desc_sw128(tc::smem_u32(sm + SM::B + sb * (N * 128)));
+              const uint32_t b_addr = tc::smem_u32(sm + SM::B + sb * (N * 128)) + b_col;
+              tc::wgmma_fence();
 #pragma unroll
               for (int k = 0; k < 4; k++)
-                tc::umma_f16_lead(d_tmem, a_desc + (uint64_t)(dy * (CG_TW * 128 / 16) + k * 2), b_desc + (uint64_t)(k * 2), idesc,
-                                  (u | dy | k) ? 1u : 0u, lead);
-              tc::umma_commit_lead(&empty_b[sb], lead);
+#pragma unroll
+                for (int ps = 0; ps < PASSES; ps++) {
+                  const uint64_t bd = tc::desc_sw128(b_addr + ps * CPP * 128 + k * 32);
+#pragma unroll
+                  for (int hf = 0; hf < 2; hf++)
+                    tc::wgmma_f16<GC>(acc[ps][hf], tc::desc_sw128(a_addr + dy * 2048 + hf * 8192 + k * 32), bd,
+                                      (u | dy | k) ? 1u : 0u);
+                }
+              tc::wgmma_commit();
             }
-            tc::umma_commit_lead(&empty_a[sa], lead);
+            tc::wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) {
+#pragma unroll
+              for (int dy = 0; dy < 3; dy++) tc::mbar_arrive(&empty_b[sbs[dy]]);
+              tc::mbar_arrive(&empty_a[sa]);
+            }
           }
         } else {
           for (int kb = 0; kb < nkb; kb++, it++) {
             const int st = it % CG_STAGES, ph = (it / CG_STAGES) & 1;
             tc::mbar_wait(&full_b[st], ph);
-            tc::tc_fence_after();
-            const uint64_t a_desc = tc::umma_desc_sw128(tc::smem_u32(sm + SM::A + st * 16384));
-            const uint64_t b_desc = tc::umma_desc_sw128(tc::smem_u32(sm + SM::B + st * (N * 128)));
+            const uint32_t a_addr = tc::smem_u32(sm + SM::A + st * 16384);
+            const uint32_t b_addr = tc::smem_u32(sm + SM::B + st * (N * 128)) + b_col;
+            tc::wgmma_fence();
 #pragma unroll
             for (int k = 0; k < 4; k++)
-              tc::umma_f16_lead(d_tmem, a_desc + (uint64_t)(k * 2), b_desc + (uint64_t)(k * 2), idesc, (kb | k) ? 1u : 0u, lead);
-            tc::umma_commit_lead(&empty_b[st], lead);
+#pragma unroll
+              for (int ps = 0; ps < PASSES; ps++) {
+                const uint64_t bd = tc::desc_sw128(b_addr + ps * CPP * 128 + k * 32);
+#pragma unroll
+                for (int hf = 0; hf < 2; hf++)
+                  tc::wgmma_f16<GC>(acc[ps][hf], tc::desc_sw128(a_addr + hf * 8192 + k * 32), bd, (kb | k) ? 1u : 0u);
+              }
+            tc::wgmma_commit();
+            tc::wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) tc::mbar_arrive(&empty_b[st]);
           }
         }
-        tc::umma_commit_lead(&tm_full[as], lead);
+#pragma unroll
+        for (int ps = 0; ps < PASSES; ps++) { tc::acc_fence(acc[ps][0]); tc::acc_fence(acc[ps][1]); }
       }
-    }
-  } else {
-    // ===================== epilogue: 8 warps; warp pair (w, w+4) shares a TMEM lane quarter and
-    // splits the N columns in halves (N >= 64), thread = output pixel =====================
-    const int q = warp & 3;
-    const int grp = (warp - 2) >> 2;
-    const int row = q * 32 + lane;
-    const int hh = row / CG_TW, ww = row % CG_TW;
-    const int etid = threadIdx.x - 64;
-    constexpr int NG = (N >= 64) ? N / 2 : N;       // columns per group
-    const int cbeg = (N >= 64) ? grp * NG : 0;
-    const bool works = (N >= 64) || grp == 0;
-    uint32_t tcount = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, tcount++) {
       const int n = tile / tiles_per_img, tt = tile % tiles_per_img;
       const int h0 = (tt / p.tiles_w) * CG_TH, w0 = (tt % p.tiles_w) * CG_TW;
       const int h = h0 + hh, w = w0 + ww;
@@ -221,17 +235,11 @@ conv_igemm_kernel(const __grid_constant__ ConvMaps maps, ConvParams p) {
       // mode 4 with sub == 2: only even rows/cols are kept; they are compacted to a 4x8 staging tile
       const bool kept = (MODE != 4) || (p.sub == 1) || (((hh | ww) & 1) == 0);
       const int srow = (MODE == 4 && p.sub == 2) ? (hh >> 1) * (CG_TW / 2) + (ww >> 1) : row;
-      const int as = tcount & 1, aph = (tcount >> 1) & 1;
-      tc::mbar_wait(&tm_full[as], aph);
-      tc::tc_fence_after();
       // staging buffers free again once the previous tile's TMA stores have read them
       if (MODE != 3 && etid == 0) tma_store_wait_read();
       asm volatile("bar.sync 1, 256;" ::: "memory");
-      const uint32_t taddr = tmem_base + as * ACC_STRIDE + ((uint32_t)(q * 32) << 16);
       const float* g = p.gctx ? p.gctx + (size_t)n * N : nullptr;
-      constexpr int PASSES = SM::PASSES, CPP = N / PASSES;          // columns staged per pass
-      constexpr int GC = (N >= 64) ? CPP / 2 : N;                   // columns per warp group per pass
-#pragma unroll 1
+#pragma unroll
       for (int pass = 0; pass < PASSES; pass++) {
         if (pass > 0) {
           // the staging tiles are reused: wait until the previous pass' TMA stores have read them
@@ -240,11 +248,17 @@ conv_igemm_kernel(const __grid_constant__ ConvMaps maps, ConvParams p) {
         }
         const int cbeg = pass * CPP + ((N >= 64) ? grp * GC : 0);
         if (works) {
-#pragma unroll 1
+#pragma unroll
           for (int c0 = cbeg; c0 < cbeg + GC; c0 += 32) {
             uint32_t r[32];
-            tc::tmem_ld_32x32(taddr + c0, r);
-            // operand loads of the gating modes overlap the TMEM read
+            // accumulator columns c0 .. c0+31 of this warpgroup -> row of this thread
+            const int j0 = (c0 - cbeg) / 8;
+            tc::named_sync(5 + grp, 128);
+            tc::acc_to_smem<GC>(scr, CG_SCR_LD, 0, 0, acc[pass][0], wtid, j0, j0 + 4);
+            tc::acc_to_smem<GC>(scr, CG_SCR_LD, 64, 0, acc[pass][1], wtid, j0, j0 + 4);
+            tc::named_sync(5 + grp, 128);
+            tc::smem_row_ld<32>(scr, CG_SCR_LD, row, 0, r);
+            // operand loads of the gating modes overlap the accumulator read
             uint4 an[4] = {}, az[4] = {};
             if (MODE == 1) {
               if (c0 >= 128 && valid) {
@@ -264,12 +278,11 @@ conv_igemm_kernel(const __grid_constant__ ConvMaps maps, ConvParams p) {
                 }
               }
             }
-            tc::tmem_ld_wait();
             float v[32];
             epi_chunk<MODE>(r, v, sbias, g, c0, p.act, valid, an, az);
             if (MODE == 3) {
               const float cs = warp_colsum32(v, lane);
-              atomicAdd(&sacc[c0 + lane], cs);
+              p.partials[((size_t)tile * 4 + q) * N + c0 + lane] = cs;     // (tile, row quarter, column)
             } else {
               // fp16, into the staging tile of this 64-channel group (tile index within the pass)
               const int t64 = (c0 - pass * CPP) / 64;
@@ -302,16 +315,11 @@ conv_igemm_kernel(const __grid_constant__ ConvMaps maps, ConvParams p) {
                   v[i] = hv; q2[i] = hv * hv;
                 }
                 const float cs = warp_colsum32(v, lane), cq = warp_colsum32(q2, lane);
-                if (c0 + lane < N) { atomicAdd(&sacc[c0 + lane], cs); atomicAdd(&sacc[N + c0 + lane], cq); }
+                if (c0 + lane < N)
+                  *reinterpret_cast<float2*>(p.partials + (((size_t)tile * 4 + q) * N + c0 + lane) * 2) = make_float2(cs, cq);
               }
             }
           }
-        }
-        if (pass == PASSES - 1) {
-          // the accumulator stage may be overwritten by the next tile's MMAs
-          tc::tc_fence_before();
-          __syncwarp();
-          if (lane == 0) tc::mbar_arrive(&tm_empty[as]);
         }
         if (MODE != 3) {
           tc::fence_proxy_async();
@@ -332,30 +340,34 @@ conv_igemm_kernel(const __grid_constant__ ConvMaps maps, ConvParams p) {
           }
         }
       }
-      if (MODE != 3) {
-        if (MODE == 4 && p.stats) {
-          // flush this tile's channel statistics (shared accumulators were completed before the last bar.sync 2)
-          for (int i = etid; i < 2 * N; i += 32 * CG_EPI_WARPS) {
-            const float sv = sacc[i];
-            sacc[i] = 0.f;
-            if (sv != 0.f) atomicAdd(p.stats + ((size_t)n * N + (i % N)) * 2 + (i / N), sv);
-          }
-        }
-      } else {
-        // flush this tile's column sums (the next tile usually belongs to another image)
-        asm volatile("bar.sync 2, 256;" ::: "memory");
-        if (etid < N) {
-          const float sv = sacc[etid];
-          sacc[etid] = 0.f;
-          if (sv != 0.f) atomicAdd(p.gsum + (size_t)n * 128 + etid, sv);
-        }
-      }
     }
     if (MODE != 3 && etid == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
   }
-  tc::tc_fence_before();
+}
+
+// Per-tile partial sums -> per-image sums in a FIXED order (tiles of the image in order, row quarters in order), so
+// that the result does not depend on which CTA ran which tile: partials [B][T][4][N][K] -> out[b][c][k] +=
+// (out row stride `ld` columns).  Block = 32 (column, k) entries x 8 tile lanes; lane l takes tiles l, l+8, ...
+__global__ void __launch_bounds__(256)
+conv_partials_reduce_kernel(const float* __restrict__ partials, float* __restrict__ out, int T, int N, int K, int ld) {
+  __shared__ float red[8][33];
+  const int b = blockIdx.y, ck = blockIdx.x * 32 + (threadIdx.x & 31), l = threadIdx.x >> 5;
+  const int NK = N * K;
+  float s = 0.f;
+  if (ck < NK) {
+    for (int t = l; t < T; t += 8) {
+      const float* pt = partials + ((size_t)b * T + t) * 4 * NK + ck;
+      s += ((pt[0] + pt[NK]) + pt[2 * NK]) + pt[3 * NK];
+    }
+  }
+  red[l][threadIdx.x & 31] = s;
   __syncthreads();
-  if (warp == 1) tc::tmem_dealloc<TCOLS>(tmem_base);
+  if (l == 0 && ck < NK) {
+    float v = red[0][threadIdx.x];
+#pragma unroll
+    for (int i = 1; i < 8; i++) v += red[i][threadIdx.x];
+    out[(size_t)b * ld * K + ck] += v;
+  }
 }
 
 template <int N, int MODE, bool HALO>
@@ -418,7 +430,8 @@ extern "C" {
 int nslam_conv_igemm_ex(const void* const* srcs, const int* src_channels, int n_src, int B, int H, int W,
                         int KH, int KW, int pad, int N, const void* wpacked, const float* bias, int mode,
                         int act, const float* gctx, const void* net, const void* zbuf, float* gsum,
-                        void* out0, int out0_channels, void* out1, float* stats, int sub, int num_sms, void* stream) {
+                        void* out0, int out0_channels, void* out1, float* stats, int sub, float* partials, int num_sms,
+                        void* stream) {
   using namespace nslam;
   if (n_src < 1 || n_src > 4 || B <= 0) return (int)cudaErrorInvalidValue;
   ConvMaps maps;
@@ -427,13 +440,11 @@ int nslam_conv_igemm_ex(const void* const* srcs, const int* src_channels, int n_
   p.tiles_h = (H + CG_TH - 1) / CG_TH; p.tiles_w = (W + CG_TW - 1) / CG_TW;
   p.n_src = n_src; p.KH = KH; p.KW = KW; p.pad = pad; p.N = N; p.mode = mode; p.act = act;
   p.wpacked = (const __half*)wpacked; p.bias = bias; p.gctx = gctx; p.net = (const __half*)net;
-  p.zbuf = (const __half*)zbuf; p.gsum = gsum; p.stats = stats; p.sub = (mode == 4 && sub == 2) ? 2 : 1;
+  p.zbuf = (const __half*)zbuf; p.gsum = gsum; p.stats = stats; p.partials = partials; p.sub = (mode == 4 && sub == 2) ? 2 : 1;
+  const bool reduce = (mode == 3) || (mode == 4 && stats != nullptr);
+  if (reduce && partials == nullptr) return (int)cudaErrorInvalidValue;
   if (mode == 4 && sub != 1 && sub != 2) return (int)cudaErrorInvalidValue;
-  // NSLAM_CONV_HALO=1: the 16x16 super-tile kernel with one halo box per channel block (conv_halo.cu) for 3x3 / pad 1,
-  // epilogue modes 0-2 — parity-green but not faster on a B200 (profiles/r02_conv_analysis.md); measurement switch.
-  static const bool want_halo2 = [] { const char* e = std::getenv("NSLAM_CONV_HALO"); return e && e[0] == '1'; }();
-  const bool halo2 = want_halo2 && !conv_pairs_enabled() && conv_halo_supported(N, mode, KH, KW, pad);
-  // first generation, 3x3 / pad 1: column-shifted halo tiles (see CgSmem); everything else: one tile per tap
+  // 3x3 / pad 1: column-shifted halo tiles (see CgSmem); everything else: one tile per tap
   const bool halo = (KH == 3 && KW == 3 && pad == 1 && mode != 3);
   int cbt = 0;
   for (int s = 0; s < n_src; s++) {
@@ -444,7 +455,6 @@ int nslam_conv_igemm_ex(const void* const* srcs, const int* src_channels, int n_
     uint64_t dims[4] = {(uint64_t)C, (uint64_t)W, (uint64_t)H, (uint64_t)B};
     uint64_t strides[3] = {(uint64_t)C * 2, (uint64_t)W * C * 2, (uint64_t)H * W * C * 2};
     uint32_t box[4] = {64, CG_TW, (uint32_t)(halo ? CG_TH + 2 : CG_TH), 1};
-    if (halo2) { box[1] = CH2_BOX; box[2] = CH2_BOX; }
     int r = tc::make_tmap_f16(&maps.src[s], srcs[s], 4, dims, strides, box);
     if (r) return r;
   }
@@ -458,25 +468,26 @@ int nslam_conv_igemm_ex(const void* const* srcs, const int* src_channels, int n_
       uint64_t dims[4] = {(uint64_t)C, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)B};
       uint64_t strides[3] = {(uint64_t)C * 2, (uint64_t)Wo * C * 2, (uint64_t)Ho * Wo * C * 2};
       uint32_t box[4] = {(uint32_t)(C < 64 ? C : 64), (uint32_t)(CG_TW / p.sub), (uint32_t)(CG_TH / p.sub), 1};
-      if (halo2) { box[1] = 8; box[2] = 16; }                    // sub-tile of the second-generation kernel
       int r = tc::make_tmap_f16(&maps.out[o], outs[o], 4, dims, strides, box, false, nullptr, /*swizzle128=*/N >= 64);
       if (r) return r;
     }
   }
-  if (halo2) {
-    p.tiles_h = (H + 15) / 16; p.tiles_w = (W + 15) / 16;        // super-tiles
-    return launch_conv_halo(N, maps, p, num_sms, (cudaStream_t)stream);
-  }
-  if (conv_pairs_enabled() && conv_pairs_supported(N, mode, halo)) return launch_conv_pairs(N, maps, p, num_sms, (cudaStream_t)stream);
-  return launch_conv(N, maps, p, halo, num_sms, (cudaStream_t)stream);
+  int r = launch_conv(N, maps, p, halo, num_sms, (cudaStream_t)stream);
+  if (r || !reduce) return r;
+  const int K = (mode == 3) ? 1 : 2;
+  const dim3 grid((N * K + 31) / 32, B);
+  conv_partials_reduce_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(partials, mode == 3 ? gsum : stats,
+                                                                      p.tiles_h * p.tiles_w, N, K, mode == 3 ? 128 : N);
+  NSLAM_CHECK_LAUNCH();
+  return 0;
 }
 
 int nslam_conv_igemm(const void* const* srcs, const int* src_channels, int n_src, int B, int H, int W,
                      int KH, int KW, int pad, int N, const void* wpacked, const float* bias, int mode,
                      int act, const float* gctx, const void* net, const void* zbuf, float* gsum,
-                     void* out0, int out0_channels, void* out1, int num_sms, void* stream) {
+                     void* out0, int out0_channels, void* out1, float* partials, int num_sms, void* stream) {
   return nslam_conv_igemm_ex(srcs, src_channels, n_src, B, H, W, KH, KW, pad, N, wpacked, bias, mode, act, gctx, net, zbuf,
-                             gsum, out0, out0_channels, out1, nullptr, 1, num_sms, stream);
+                             gsum, out0, out0_channels, out1, nullptr, 1, partials, num_sms, stream);
 }
 
 }  // extern "C"

@@ -11,7 +11,7 @@
 //     (c10::Half arithmetic goes through fp32 and rounds after every operator), which is
 //     what __hmul_rn/__hadd_rn compute => the fp16 path is bit-exact w.r.t. the reference.
 //
-// B200 design: instead of 4 launches that zero-fill the output and then issue up to 256
+// Design: instead of 4 launches that zero-fill the output and then issue up to 256
 // global read-modify-writes per thread, one launch covers all levels; each thread gathers its
 // (2r+2)^2 taps into registers with independent loads (64 requests in flight per thread),
 // combines them in registers and writes each output channel exactly once (coalesced along x).
@@ -103,7 +103,7 @@ corr_lookup_kernel(LookupLevels lv, const float* __restrict__ coords, T* __restr
   const T w00 = Arith<T>::cvt((1.0f - dx) * (1.0f - dy));
 
   // output: reference layout [n][L*RD*RD][h1][w1], or channels-last [n][h1][w1][nhwc_stride]
-  // (operand layout of the tcgen05 convolution; channels >= L*RD*RD are zero-filled by level 0)
+  // (operand layout of the wgmma convolution; channels >= L*RD*RD are zero-filled by level 0)
   const size_t ostride = nhwc_stride ? 1 : (size_t)hw;
   T* __restrict__ o = nhwc_stride
                           ? out + ((size_t)n * hw + p) * nhwc_stride + (size_t)l * (RD * RD)
@@ -205,10 +205,10 @@ corr_lookup_nhwc_kernel(LookupLevels lv, const float* __restrict__ coords, T* __
     *reinterpret_cast<uint4*>(dst + b) = *reinterpret_cast<const uint4*>(src + b);
 }
 
-// (Round 2 tried a 128-bit variant of the kernel above — aligned 16-byte chunk pairs + a select network on levels 0/1,
-// the CTA's contiguous level-2/3 slices staged in shared memory.  Bit-identical output, but 74 us instead of 56 us per
-// update() at 18 edges on a B200 (profiles/r02_kernel_table_call5_*): the two-byte gathers already coalesce into the
-// same 32-byte sectors, and the select network costs more issue slots than the gathers it replaces.  Removed.)
+// (A 128-bit variant of the kernel above — aligned 16-byte chunk pairs + a select network on levels 0/1, the CTA's
+// contiguous level-2/3 slices staged in shared memory — gave bit-identical output but was slower: the two-byte gathers
+// already coalesce into the same 32-byte sectors, and the select network costs more issue slots than the gathers it
+// replaces.  Removed.)
 
 template <typename T>
 static int launch_lookup(const LookupLevels& lv, const float* coords, void* out, int n, int h1,

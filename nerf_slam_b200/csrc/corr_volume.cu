@@ -8,12 +8,13 @@
 // pooling kernels that each re-read the previous level, and `CorrBlock.cat` re-copies the whole
 // pool on every add.  The op is HBM-write bound (AI ~93 FLOP/B, SURVEY.md §8d: 63.6 MB/edge).
 //
-// B200 design: per CTA one (edge, 128-source-pixel) strip.  A (128 px x C=128, fp16) is loaded once
+// Design: per CTA one (edge, 128-source-pixel) strip.  A (128 px x C=128, fp16) is loaded once
 // by TMA; the CTA then walks the target image in 8x16-pixel tiles: TMA brings the 128x128 B tile
-// (box {64c,16w,8h}, SWIZZLE_128B, OOB rows zero-filled) through a 3-stage mbarrier ring, one
-// thread issues 8 tcgen05.mma (M128 N128 K16, fp32 accumulators in TMEM, double buffered), and
-// four epilogue warps read the accumulators with tcgen05.ld, scale by 1/16, round to fp16 and
-// build pyramid levels 1..3 from the SAME registers (an 8x16 target tile contains complete
+// (box {64c,16w,8h}, SWIZZLE_128B, OOB rows zero-filled) through a 2-stage mbarrier ring.  Two
+// warpgroups take alternate tiles (one computes while the other stores): each issues 2 x 8 wgmma
+// (M64 N128 K16, fp32 accumulators in registers), passes the accumulators through a 32-column fp32
+// shared tile so that thread = source pixel, scales by 1/16, rounds to fp16 and
+// builds pyramid levels 1..3 from the SAME registers (an 8x16 target tile contains complete
 // 2x2/4x4/8x8 pooling cells; the fp16 rounding chain of the reference is reproduced), stage the
 // four tiles in shared memory and write every level once: levels 0/1 with one TMA store per tile
 // ({16,8,128} box straight from the staging buffer), levels 2/3 with cooperative stores.
@@ -23,8 +24,9 @@
 
 namespace nslam {
 
-constexpr int CV_STAGES = 3;
-constexpr int CV_THREADS = 320;            // TMA warp, MMA warp, 2 epilogue groups of 4 warps
+constexpr int CV_STAGES = 2;
+constexpr int CV_THREADS = 288;            // 2 warpgroups (MMA + epilogue), TMA warp
+constexpr int CV_SCR_LD = 40;              // fp32 accumulator chunk [128][32 + 8 padding]
 constexpr int CV_TH = 8, CV_TW = 16;       // target tile
 constexpr int CV_L0_STRIDE = 256;          // bytes per staged row: dense [8][16] halfs = the TMA store box
 constexpr int CV_L1_STRIDE = 64;           // dense [4][8]
@@ -41,8 +43,10 @@ struct CvSmem {
   static constexpr int L1 = L0 + 128 * CV_L0_STRIDE;
   static constexpr int L2 = L1 + 128 * CV_L1_STRIDE;
   static constexpr int L3 = L2 + 128 * CV_L2_STRIDE;
-  static constexpr int BAR = ST + 2 * CV_STAGE_BYTES;  // mbarriers
+  static constexpr int SCR = ST + 2 * CV_STAGE_BYTES;  // 2 warpgroups x [128][CV_SCR_LD] fp32
+  static constexpr int BAR = SCR + 2 * 128 * CV_SCR_LD * 4;  // mbarriers
   static constexpr int TOTAL = BAR + 128;
+  static_assert(TOTAL + 1024 <= 227 * 1024, "shared memory plan");
 };
 
 struct CvParams {
@@ -106,8 +110,8 @@ __device__ __forceinline__ void cv_store_level(const unsigned char* stage, int r
 }
 
 // Persistent kernel: grid = min(#SMs, nwork).  Work item = (edge, 128-source-pixel strip); the
-// B-tile ring, the TMEM accumulator stages and the two epilogue groups run across work items
-// without draining (global tile counter t: ring slot = t % STAGES, epilogue group = t & 1).
+// B-tile ring and the two warpgroups run across work items without draining (global tile counter t:
+// ring slot = t % STAGES, warpgroup = t & 1).
 __global__ void __launch_bounds__(CV_THREADS, 1)
 corr_volume_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                       const __grid_constant__ CUtensorMap tmO0, const __grid_constant__ CUtensorMap tmO1, CvParams p) {
@@ -119,29 +123,21 @@ corr_volume_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
   uint64_t* empty_b = bars + CV_STAGES;       // [STAGES]
   uint64_t* a_full = bars + 2 * CV_STAGES;    // [1]
   uint64_t* a_empty = a_full + 1;             // [1]
-  uint64_t* tm_full = a_empty + 1;            // [2]
-  uint64_t* tm_empty = tm_full + 2;           // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tm_empty + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int NT = p.NH * p.NW;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tc::tma_prefetch_desc(&tmA);
     tc::tma_prefetch_desc(&tmB);
-    for (int s = 0; s < CV_STAGES; s++) { tc::mbar_init(&full_b[s], 1); tc::mbar_init(&empty_b[s], 1); }
+    for (int s = 0; s < CV_STAGES; s++) { tc::mbar_init(&full_b[s], 1); tc::mbar_init(&empty_b[s], 4); }
     tc::mbar_init(a_full, 1);
-    tc::mbar_init(a_empty, 1);
-    for (int s = 0; s < 2; s++) { tc::mbar_init(&tm_full[s], 1); tc::mbar_init(&tm_empty[s], 4); }
+    tc::mbar_init(a_empty, 8);                // every warp of both warpgroups, once per strip
     tc::fence_barrier_init();
   }
-  if (warp == 1) tc::tmem_alloc<256>(tmem_slot);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       uint32_t t = 0, wi = 0;
@@ -165,61 +161,51 @@ corr_volume_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = tc::umma_idesc_f16(128, 128, 0);
-      const uint32_t a_addr = tc::smem_u32(sm + CvSmem::A);
-      uint32_t t = 0, wi = 0;
-      for (int w = blockIdx.x; w < p.nwork; w += gridDim.x, wi++) {
-        const int ck = w % p.split;
-        const int n_lo = ck * NT / p.split, n_hi = (ck + 1) * NT / p.split;
-        tc::mbar_wait(a_full, wi & 1);
-        for (int n = n_lo; n < n_hi; n++, t++) {
-          const int s = t % CV_STAGES, ph = (t / CV_STAGES) & 1;
-          const int as = t & 1, aph = (t >> 1) & 1;
-          tc::mbar_wait(&tm_empty[as], aph ^ 1);
-          tc::mbar_wait(&full_b[s], ph);
-          tc::tc_fence_after();
-          const uint32_t b_addr = tc::smem_u32(sm + CvSmem::B + s * 32768);
-          const uint32_t d_tmem = tmem_base + as * 128;
-#pragma unroll
-          for (int kh = 0; kh < 2; kh++) {
-#pragma unroll
-            for (int k = 0; k < 4; k++) {
-              const uint64_t ad = tc::umma_desc_sw128(a_addr + kh * 16384 + k * 32);
-              const uint64_t bd = tc::umma_desc_sw128(b_addr + kh * 16384 + k * 32);
-              tc::umma_f16(d_tmem, ad, bd, idesc, (kh | k) ? 1u : 0u);
-            }
-          }
-          tc::umma_commit(&empty_b[s]);
-          tc::umma_commit(&tm_full[as]);
-        }
-        tc::umma_commit(a_empty);
-      }
-    }
   } else {
-    // ===================== epilogue: 2 groups x 4 warps, thread <-> accumulator row =====================
-    const int grp = (warp - 2) >> 2;      // group g serves tiles with (t & 1) == g == TMEM stage g
-    const int q = warp & 3;               // TMEM lane quarter accessible by this warp
-    const int row = q * 32 + lane;        // row inside the 128-row strip
-    const int etid = ((warp - 2) & 3) * 32 + lane;
+    // ===================== 2 warpgroups: MMA + epilogue, thread <-> accumulator row =====================
+    const int grp = warp >> 2;            // warpgroup g serves tiles with (t & 1) == g
+    const int etid = threadIdx.x & 127;
+    const int row = etid;                 // row inside the 128-row strip
     unsigned char* stg = sm + CvSmem::ST + grp * CV_STAGE_BYTES;
     unsigned char* st0 = stg + CvSmem::L0 + row * CV_L0_STRIDE;
     unsigned char* st1 = stg + CvSmem::L1 + row * CV_L1_STRIDE;
     unsigned char* st2 = stg + CvSmem::L2 + row * CV_L2_STRIDE;
     unsigned char* st3 = stg + CvSmem::L3 + row * CV_L3_STRIDE;
-    const uint32_t taddr = tmem_base + grp * 128 + ((uint32_t)(q * 32) << 16);
-    uint32_t t = 0, use = 0;
-    for (int w = blockIdx.x; w < p.nwork; w += gridDim.x) {
+    float* scr = reinterpret_cast<float*>(sm + CvSmem::SCR) + grp * 128 * CV_SCR_LD;
+    const uint32_t a_addr = tc::smem_u32(sm + CvSmem::A);
+    uint32_t t = 0, wi = 0;
+    for (int w = blockIdx.x; w < p.nwork; w += gridDim.x, wi++) {
       const int ws = w / p.split, ck = w % p.split;
       const int e = ws / p.MT, m0 = (ws % p.MT) * 128;
       const int n_lo = ck * NT / p.split, n_hi = (ck + 1) * NT / p.split;
+      tc::mbar_wait(a_full, wi & 1);
       for (int n = n_lo; n < n_hi; n++, t++) {
         if ((int)(t & 1) != grp) continue;
-        tc::mbar_wait(&tm_full[grp], use & 1);
-        use++;
-        tc::tc_fence_after();
+        const int s = t % CV_STAGES, ph = (t / CV_STAGES) & 1;
+        tc::mbar_wait(&full_b[s], ph);
+        float acc[2][64];
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+          for (int i = 0; i < 64; i++) acc[h][i] = 0.f;
+        const uint32_t b_addr = tc::smem_u32(sm + CvSmem::B + s * 32768);
+        tc::wgmma_fence();
+#pragma unroll
+        for (int kh = 0; kh < 2; kh++) {
+#pragma unroll
+          for (int k = 0; k < 4; k++) {
+            const uint64_t bd = tc::desc_sw128(b_addr + kh * 16384 + k * 32);
+#pragma unroll
+            for (int h = 0; h < 2; h++)
+              tc::wgmma_f16<128>(acc[h], tc::desc_sw128(a_addr + kh * 16384 + h * 8192 + k * 32), bd, (kh | k) ? 1u : 0u);
+          }
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::acc_fence(acc[0]);
+        tc::acc_fence(acc[1]);
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&empty_b[s]);     // B stage free for the next TMA load
         // this group's staging buffers are free once its previous tile's stores have read them
         if (etid == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
         if (grp == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
@@ -228,8 +214,12 @@ corr_volume_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
 #pragma unroll
         for (int c = 0; c < 4; c++) {
           uint32_t r[32];
-          tc::tmem_ld_32x32(taddr + c * 32, r);
-          tc::tmem_ld_wait();
+          // accumulator columns 32c .. 32c+31 (target rows 2c, 2c+1 of the tile) of every strip row
+          if (c > 0) tc::named_sync(5 + grp, 128);
+          tc::acc_to_smem<128>(scr, CV_SCR_LD, 0, 0, acc[0], etid, 4 * c, 4 * c + 4);
+          tc::acc_to_smem<128>(scr, CV_SCR_LD, 64, 0, acc[1], etid, 4 * c, 4 * c + 4);
+          tc::named_sync(5 + grp, 128);
+          tc::smem_row_ld<32>(scr, CV_SCR_LD, row, 0, r);
           __half h[32];
 #pragma unroll
           for (int i = 0; i < 32; i++) h[i] = __float2half_rn(__uint_as_float(r[i]) * 0.0625f);
@@ -246,10 +236,7 @@ corr_volume_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
           }
           *reinterpret_cast<uint4*>(st1 + c * 16) = *reinterpret_cast<const uint4*>(l1[c]);
         }
-        // accumulator stage can be overwritten by the next MMA
-        tc::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) tc::mbar_arrive(&tm_empty[grp]);
+        tc::named_sync(5 + grp, 128);                      // chunk tile free for the next tile of this group
         __half l2[2][4];
 #pragma unroll
         for (int c2 = 0; c2 < 2; c2++) {
@@ -291,12 +278,11 @@ corr_volume_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         cv_store_level<2, 1>(stg + CvSmem::L3, CV_L3_STRIDE, p.out[3], e, p.HW, m0, p.H2 >> 3,
                              p.W2 >> 3, h0 >> 3, w0 >> 3, etid);
       }
+      __syncwarp();
+      if (lane == 0) tc::mbar_arrive(a_empty);             // this warp's MMAs of the strip are complete
     }
     if (etid == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tc::tmem_dealloc<256>(tmem_base);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -362,7 +348,7 @@ int nslam_corr_volume_build(const void* fmaps, int NF, int H, int W, int C, cons
   p.ii = ii; p.jj = jj; p.HW = HW; p.H2 = H; p.W2 = W;
   p.NH = (H + CV_TH - 1) / CV_TH; p.NW = (W + CV_TW - 1) / CV_TW;
   p.MT = (HW + 127) / 128;
-  int dev0 = 0, sms0 = 148;
+  int dev0 = 0, sms0 = 132;
   cudaGetDevice(&dev0);
   cudaDeviceGetAttribute(&sms0, cudaDevAttrMultiProcessorCount, dev0);
   // few edges (the per-frame motion filter builds ONE volume): split the target tiles of a strip over
@@ -394,7 +380,7 @@ int nslam_corr_volume_build(const void* fmaps, int NF, int H, int W, int C, cons
     if (er != cudaSuccess) return (int)er;
     configured = true;
   }
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int grid = p.nwork < sms ? p.nwork : sms;

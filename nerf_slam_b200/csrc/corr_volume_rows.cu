@@ -10,18 +10,19 @@
 // (6 % of the bytes).  The fp16 rounding chain of the reference (each level rounded, pooled from the previous
 // fp16 level, summation order (h0,w0),(h0,w1),(h1,w0),(h1,w1)) is kept.
 //
-// Pipeline: persistent CTAs over (edge, 128-source-pixel strip, chunk of row pairs [multiple of 4]); warp 0 = TMA
-// producer (A strip once per item, B = 2W2 x 128 channels per row pair, 3-stage ring), warp 1 = MMA issuer
-// (8 x tcgen05.mma M128 x N(2W2) x K16 into one of two TMEM stages), warps 2..9 = epilogue: the two warps of a
-// TMEM lane quarter split the columns in halves (w < W2/2 | w >= W2/2), thread = source pixel.
+// Pipeline: persistent CTAs over (edge, 128-source-pixel strip, chunk of row pairs [multiple of 4]); warp 8 = TMA
+// producer (A strip once per item, B = 2W2 x 128 channels per row pair, 2-stage ring), warps 0..7 = two warpgroups
+// that split the columns in halves (w < W2/2 | w >= W2/2): each issues its wgmmas (M64 x N(W2/2) x K16, both target
+// rows, both 64-row halves of the strip), then passes the fp32 accumulators through the B stage it has just consumed
+// so that thread = source pixel, and runs the epilogue.
 // Requirements: C = 128, W2 % 16 == 0, 2*W2 <= 192, H2 even.  tests/test_gpu_parity.py::test_corr_volume_rows_*.
 #include "common.cuh"
 #include "tc.cuh"
 
 namespace nslam {
 
-constexpr int CR_THREADS = 320;
-constexpr int CR_STAGES = 2;      // the epilogue / store path bounds the kernel (MMAs: 640 of ~2500 cycles per tile)
+constexpr int CR_THREADS = 288;
+constexpr int CR_STAGES = 2;      // the epilogue / store path bounds the kernel
 
 struct CrParams {
   __half* out[4];
@@ -73,23 +74,15 @@ corr_volume_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
   uint64_t* empty_b = bars + CR_STAGES;
   uint64_t* a_full = bars + 2 * CR_STAGES;
   uint64_t* a_empty = a_full + 1;
-  uint64_t* tm_full = a_empty + 1;
-  uint64_t* tm_empty = tm_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tm_empty + 2);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tc::tma_prefetch_desc(&tmA); tc::tma_prefetch_desc(&tmB);
-    for (int s = 0; s < CR_STAGES; s++) { tc::mbar_init(&full_b[s], 1); tc::mbar_init(&empty_b[s], 1); }
-    tc::mbar_init(a_full, 1); tc::mbar_init(a_empty, 1);
-    for (int s = 0; s < 2; s++) { tc::mbar_init(&tm_full[s], 1); tc::mbar_init(&tm_empty[s], 8); }
+    for (int s = 0; s < CR_STAGES; s++) { tc::mbar_init(&full_b[s], 1); tc::mbar_init(&empty_b[s], 8); }
+    tc::mbar_init(a_full, 1); tc::mbar_init(a_empty, 8);
     tc::fence_barrier_init();
   }
-  if (warp == 1) tc::tmem_alloc<512>(tmem_slot);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   // work item w -> (edge, strip, row-pair range)
   auto item = [&](int w, int& e, int& m0, int& rp_lo, int& rp_hi) {
@@ -98,7 +91,7 @@ corr_volume_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
     rp_lo = ck * p.rp_chunk; rp_hi = min(p.RP, rp_lo + p.rp_chunk);
   };
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       uint32_t t = 0, wi = 0;
       for (int w = blockIdx.x; w < p.nwork; w += gridDim.x, wi++) {
@@ -119,72 +112,70 @@ corr_volume_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = tc::umma_idesc_f16(128, NB, 0);
-      const uint32_t a_addr = tc::smem_u32(sm + SM::A);
-      uint32_t t = 0, wi = 0;
-      for (int w = blockIdx.x; w < p.nwork; w += gridDim.x, wi++) {
-        int e, m0, rp_lo, rp_hi;
-        item(w, e, m0, rp_lo, rp_hi);
-        tc::mbar_wait(a_full, wi & 1);
-        for (int rp = rp_lo; rp < rp_hi; rp++, t++) {
-          const int s = t % CR_STAGES, ph = (t / CR_STAGES) & 1;
-          const int as = t & 1, aph = (t >> 1) & 1;
-          tc::mbar_wait(&tm_empty[as], aph ^ 1);
-          tc::mbar_wait(&full_b[s], ph);
-          tc::tc_fence_after();
-          const uint32_t b_addr = tc::smem_u32(sm + SM::B + s * SM::BSTAGE);
-          const uint32_t d_tmem = tmem_base + as * 256;
-#pragma unroll
-          for (int kh = 0; kh < 2; kh++)
-#pragma unroll
-            for (int k = 0; k < 4; k++)
-              tc::umma_f16(d_tmem, tc::umma_desc_sw128(a_addr + kh * 16384 + k * 32),
-                           tc::umma_desc_sw128(b_addr + kh * (NB * 128) + k * 32), idesc, (kh | k) ? 1u : 0u);
-          tc::umma_commit(&empty_b[s]);
-          tc::umma_commit(&tm_full[as]);
-        }
-        tc::umma_commit(a_empty);
-      }
-    }
   } else {
-    const int q = warp & 3;                      // TMEM lane quarter of this warp
-    const int hsel = (warp - 2) >> 2;            // column half
-    const int row = q * 32 + lane;
-    const int etid = threadIdx.x - 64;
+    const int hsel = warp >> 2;                  // column half = warpgroup
+    const int row = threadIdx.x & 127;
+    const int etid = threadIdx.x;
     const int c0 = hsel * WH;
     const int H2l = p.H2 >> 2, H3l = p.H2 >> 3;
-    uint32_t t = 0;
-    for (int w = blockIdx.x; w < p.nwork; w += gridDim.x) {
+    const uint32_t a_addr = tc::smem_u32(sm + SM::A);
+    uint32_t t = 0, wi = 0;
+    for (int w = blockIdx.x; w < p.nwork; w += gridDim.x, wi++) {
       int e, m0, rp_lo, rp_hi;
       item(w, e, m0, rp_lo, rp_hi);
       const int m = m0 + row;
       const bool mok = m < p.HW;
       const int eo = p.slots ? p.slots[e] : e;      // where this edge's volumes live (CorrPool slot)
       __half l1p[WH / 2], l2p[WH / 4];           // carries: level 1 of the previous (even) row pair, level 2 of the previous (even) quad
+      tc::mbar_wait(a_full, wi & 1);
       for (int rp = rp_lo; rp < rp_hi; rp++, t++) {
-        const int as = t & 1, aph = (t >> 1) & 1;
+        const int s = t % CR_STAGES, ph = (t / CR_STAGES) & 1;
         unsigned char* st0 = sm + SM::ST0 + (t & 1) * SM::ST0_BYTES + row * (NB * 2);
         unsigned char* st1 = sm + SM::ST1 + (t & 1) * SM::ST1_BYTES + row * W2;
-        tc::mbar_wait(&tm_full[as], aph);
-        tc::tc_fence_after();
-        // staging buffer t&1 is free once the store of tile t-2 has read it (at most ONE newer store group may be pending)
+        tc::mbar_wait(&full_b[s], ph);
+        unsigned char* bst = sm + SM::B + s * SM::BSTAGE;
+        const uint32_t b_addr = tc::smem_u32(bst);
+        // this warpgroup's columns: target row tr, w in [c0, c0 + WH)  (B rows tr * W2 + c0 ..)
+        float acc[2][2][WH / 2];
+#pragma unroll
+        for (int tr = 0; tr < 2; tr++)
+#pragma unroll
+          for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int i = 0; i < WH / 2; i++) acc[tr][h][i] = 0.f;
+        tc::wgmma_fence();
+#pragma unroll
+        for (int kh = 0; kh < 2; kh++)
+#pragma unroll
+          for (int k = 0; k < 4; k++)
+#pragma unroll
+            for (int tr = 0; tr < 2; tr++) {
+              const uint64_t bd = tc::desc_sw128(b_addr + kh * (NB * 128) + (tr * W2 + c0) * 128 + k * 32);
+#pragma unroll
+              for (int h = 0; h < 2; h++)
+                tc::wgmma_f16<WH>(acc[tr][h], tc::desc_sw128(a_addr + kh * 16384 + h * 8192 + k * 32), bd, (kh | k) ? 1u : 0u);
+            }
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+#pragma unroll
+        for (int tr = 0; tr < 2; tr++) { tc::acc_fence(acc[tr][0]); tc::acc_fence(acc[tr][1]); }
+        // staging buffer t&1 is free once the store of tile t-2 has read it (at most ONE newer store group may be pending);
+        // the B stage is done for both warpgroups' MMAs after this barrier and becomes the accumulator tile
         if (etid == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
         asm volatile("bar.sync 1, 256;" ::: "memory");
-        const uint32_t taddr = tmem_base + as * 256 + ((uint32_t)(q * 32) << 16);
-        // both target rows of the tile: all TMEM loads in flight, ONE wait (was: a wait per 8 columns)
+        float* scr = reinterpret_cast<float*>(bst) + hsel * 128 * WH;
         uint32_t ra[2][WH];
 #pragma unroll
         for (int tr = 0; tr < 2; tr++) {
-          tc::tmem_ld_32x32(taddr + tr * W2 + c0, ra[tr]);
-#pragma unroll
-          for (int k = 32; k < WH; k += 8) tc::tmem_ld_32x8(taddr + tr * W2 + c0 + k, ra[tr] + k);
+          if (tr) tc::named_sync(3 + hsel, 128);
+          tc::acc_to_smem<WH>(scr, WH, 0, 0, acc[tr][0], row);
+          tc::acc_to_smem<WH>(scr, WH, 64, 0, acc[tr][1], row);
+          tc::named_sync(3 + hsel, 128);
+          tc::smem_row_ld<WH>(scr, WH, row, 0, ra[tr]);
         }
-        tc::tmem_ld_wait();
-        tc::tc_fence_before();
+        tc::fence_proxy_async();
         __syncwarp();
-        if (lane == 0) tc::mbar_arrive(&tm_empty[as]);        // the accumulator stage is free for the next MMAs already
+        if (lane == 0) tc::mbar_arrive(&empty_b[s]);          // the B stage may be refilled
         __half h0[WH], h1[WH];
 #pragma unroll
         for (int tr = 0; tr < 2; tr++) {
@@ -240,12 +231,11 @@ corr_volume_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
           asm volatile("cp.async.bulk.commit_group;" ::: "memory");
         }
       }
+      __syncwarp();
+      if (lane == 0) tc::mbar_arrive(a_empty);             // this warp's MMAs of the strip are complete
     }
     if (etid == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tc::tmem_dealloc<512>(tmem_base);
 }
 
 template <int W2>
@@ -278,7 +268,7 @@ static int launch_rows(const void* fmaps, int NF, int H, const int* ii, const in
   for (int l = 0; l < 4; l++) p.out[l] = (__half*)outs[l];
   p.ii = ii; p.jj = jj; p.slots = slots; p.HW = HW; p.H2 = H; p.RP = H / 2;
   p.MT = (HW + 127) / 128;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   // chunks of row pairs (multiples of 4, so that the level-2/3 carries never cross a chunk) when E*MT < #SMs

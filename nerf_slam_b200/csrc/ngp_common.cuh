@@ -97,6 +97,14 @@ __device__ __forceinline__ uint32_t pcg(uint32_t v) {
 __device__ __forceinline__ float rnd01(uint32_t a, uint32_t b, uint32_t c) {
   return (float)(pcg(pcg(pcg(a) ^ b) ^ c) >> 8) * (1.0f / 16777216.0f);
 }
+// j-th cell (j < GRID^3) refreshed in cascade `mip` when only part of the occupancy grid is refreshed: an affine
+// permutation of the GRID^3 cells (odd multiplier, power-of-two count) with seeded coefficients, so the cells of one
+// refresh are distinct and no two threads update the same cell
+static_assert((GRID & (GRID - 1)) == 0, "GRID^3 must be a power of two");
+__device__ __forceinline__ uint32_t density_cell(uint32_t seed, int mip, int j) {
+  const uint32_t a = pcg(pcg(seed) ^ (uint32_t)(2 * mip)) | 1u, b = pcg(pcg(seed) ^ (uint32_t)(2 * mip + 1));
+  return (a * (uint32_t)j + b) & (uint32_t)(GRID * GRID * GRID - 1);
+}
 
 // ------------------------------------------------------------------ occupancy grid marching
 __device__ __forceinline__ float calc_dt(float t, float cone) {
@@ -159,3 +167,40 @@ __device__ __forceinline__ void ray_aabb(const float o[3], const float id[3], fl
 }
 
 }  // namespace ngp
+
+// ---- order-independent accumulation
+// Float atomics add in whatever order the threads arrive, so their sums differ from run to run in the last bits, and
+// training amplifies that.  Gradients that many threads scatter into the same entries are therefore accumulated as
+// 64-bit fixed-point integers (integer addition is associative) and converted to fp32 once the scatter is done.
+namespace ngp {
+__device__ __forceinline__ void fx_add(long long* acc, float v, float scale) {
+  const float x = fminf(fmaxf(v * scale, -9.2e18f), 9.2e18f);
+  atomicAdd(reinterpret_cast<unsigned long long*>(acc), (unsigned long long)__float2ll_rn(x));
+}
+// out[i] += acc[i] / scale; acc[i] = 0
+static __global__ void fx_flush_kernel(long long* __restrict__ acc, float* __restrict__ out, size_t n, float inv_scale) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const long long v = acc[i];
+    if (v != 0) { out[i] += (float)((double)v * (double)inv_scale); acc[i] = 0; }
+  }
+}
+}  // namespace ngp
+
+// library-owned device scratch, one buffer per (device, slot), grown on demand and zero-filled when (re)allocated
+inline void* ngp_scratch(int slot, size_t bytes) {
+  static void* ptr[64][4] = {};
+  static size_t cap[64][4] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= 64 || slot < 0 || slot >= 4) return nullptr;
+  if (cap[dev][slot] < bytes) {
+    if (ptr[dev][slot]) cudaFree(ptr[dev][slot]);
+    ptr[dev][slot] = nullptr; cap[dev][slot] = 0;
+    if (cudaMalloc(&ptr[dev][slot], bytes) != cudaSuccess) { ptr[dev][slot] = nullptr; return nullptr; }
+    cudaMemset(ptr[dev][slot], 0, bytes);
+    cap[dev][slot] = bytes;
+  }
+  return ptr[dev][slot];
+}
+enum { NGP_SCRATCH_GRID = 0, NGP_SCRATCH_DW = 1, NGP_SCRATCH_CAM = 2, NGP_SCRATCH_LOSS = 3 };
+

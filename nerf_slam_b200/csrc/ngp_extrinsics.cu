@@ -61,11 +61,14 @@ __device__ __forceinline__ void grid_input_grad(const float x[3], const __half2*
 }
 
 // rays [R,16] (see ngp_train.cu), coords [S,7] (unit-cube position, dt, direction), tdist [S], denc [S,32] fp16
-// cam_grad [N,6]: += (dL/d translation, dL/d rotation vector).  grid: one warp per ray.
+// cam_acc [N,6]: += (dL/d translation, dL/d rotation vector) in fixed point (CAM_FX, order-independent sums).
+// grid: one warp per ray.
+constexpr float CAM_FX = 4294967296.f;            // 2^32: fixed-point scale of the camera-gradient accumulator
+
 __global__ void __launch_bounds__(256)
 cam_grad_kernel(const float* __restrict__ rays, int n_rays, const float* __restrict__ coords,
                 const float* __restrict__ tdist, const __half* __restrict__ denc, const __half2* __restrict__ grid,
-                ExtrLevels lv, float inv_extent, float inv_loss_scale, float* __restrict__ cam_grad) {
+                ExtrLevels lv, float inv_extent, float inv_loss_scale, long long* __restrict__ cam_acc) {
   const int r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (r >= n_rays) return;
   const float* R = rays + (size_t)r * 16;
@@ -93,11 +96,11 @@ cam_grad_kernel(const float* __restrict__ rays, int n_rays, const float* __restr
   const float sc = inv_extent * inv_loss_scale;
   const float d[3] = {R[3], R[4], R[5]};
   const int img = reinterpret_cast<const int*>(R)[14];
-  float* cg = cam_grad + (size_t)img * 6;
-  atomicAdd(cg + 0, sc * go[0]); atomicAdd(cg + 1, sc * go[1]); atomicAdd(cg + 2, sc * go[2]);
-  atomicAdd(cg + 3, sc * (d[1] * gd[2] - d[2] * gd[1]));
-  atomicAdd(cg + 4, sc * (d[2] * gd[0] - d[0] * gd[2]));
-  atomicAdd(cg + 5, sc * (d[0] * gd[1] - d[1] * gd[0]));
+  long long* cg = cam_acc + (size_t)img * 6;
+  fx_add(cg + 0, sc * go[0], CAM_FX); fx_add(cg + 1, sc * go[1], CAM_FX); fx_add(cg + 2, sc * go[2], CAM_FX);
+  fx_add(cg + 3, sc * (d[1] * gd[2] - d[2] * gd[1]), CAM_FX);
+  fx_add(cg + 4, sc * (d[2] * gd[0] - d[0] * gd[2]), CAM_FX);
+  fx_add(cg + 5, sc * (d[0] * gd[1] - d[1] * gd[0]), CAM_FX);
 }
 
 // Adam on the [N,6] offsets + effective cameras.  One thread per camera.
@@ -154,17 +157,21 @@ extern "C" {
 int nslam_ngp_cam_grad(const void* grid_half, const float* scale16, const int* res16, const unsigned* size16,
                        const unsigned* offset16, const int* dense16, float aabb_scale, const float* rays, int max_rays,
                        const float* coords, const float* tdist, const void* denc, float loss_scale, float* cam_grad,
-                       void* stream) {
+                       int n_images, void* stream) {
   using namespace ngp;
   ExtrLevels lv;
   for (int l = 0; l < N_LEVELS; l++) {
     lv.scale[l] = scale16[l]; lv.res[l] = res16[l]; lv.size[l] = size16[l]; lv.offset[l] = offset16[l]; lv.dense[l] = dense16[l];
   }
-  if (max_rays <= 0) return 0;
+  if (max_rays <= 0 || n_images <= 0) return 0;
+  long long* acc = (long long*)ngp_scratch(NGP_SCRATCH_CAM, (size_t)n_images * 6 * sizeof(long long));
+  if (!acc) return (int)cudaErrorMemoryAllocation;
   const int threads = 256, warps_per_block = threads / 32;
   cam_grad_kernel<<<(max_rays + warps_per_block - 1) / warps_per_block, threads, 0, (cudaStream_t)stream>>>(
       rays, max_rays, coords, tdist, (const __half*)denc, (const __half2*)grid_half, lv, 1.f / aabb_scale, 1.f / loss_scale,
-      cam_grad);
+      acc);
+  NGX_CHECK_LAUNCH();
+  fx_flush_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(acc, cam_grad, (size_t)n_images * 6, 1.f / CAM_FX);
   NGX_CHECK_LAUNCH();
   return 0;
 }

@@ -1,14 +1,14 @@
-// Path B — tiny-MLP forward on tcgen05 tensor cores, fused with the hash-grid encoding (sm_100a).
+// Path B — tiny-MLP forward on Hopper tensor cores (wgmma), fused with the hash-grid encoding (sm_90a).
 //
 // Same function as ngp::forward_kernel (csrc/ngp_train.cu): coords -> (rgb, sigma), but the five
-// dense layers run as tcgen05.mma on a 128-sample tile:
-//   thread = sample (128 threads / CTA, persistent CTAs):
+// dense layers run as wgmma on a 128-sample tile:
+//   thread = sample (128 threads / CTA = one warpgroup, persistent CTAs):
 //     hash encode (128 independent fp16 gathers) -> row of the A tile in shared memory (fp16,
-//     K-major, 128B-swizzled) -> one thread issues M128 x N{64,16} x K16 MMAs against the layer's
-//     pre-packed weight image -> accumulator in TMEM -> tcgen05.ld of the thread's own row ->
-//     ReLU / exp / SH / sigmoid in registers -> next layer's A row ... activations never leave the SM.
+//     K-major, 128B-swizzled) -> the warpgroup issues 2 x (M64 x N{64,16} x K16) wgmmas against the
+//     layer's pre-packed weight image -> fp32 accumulator fragments -> shared fp32 tile -> the thread's
+//     own row -> ReLU / exp / SH / sigmoid in registers -> next layer's A row ... activations never leave the SM.
 // Weights: fp16 copies of the fp32 master, packed by ngp_pack_mlp_kernel after every Adam step into
-// UMMA-ready images B_l[n][k] = W_l[k][n] (K padded to 64).
+// wgmma-ready images B_l[n][k] = W_l[k][n] (K padded to 64).
 // FLOPs per sample: 2 * 10 240; roofline: tensor pipe (north_star target for the tiny MLP), in
 // practice bounded by the gather + epilogue.
 #include "ngp_common.cuh"
@@ -42,10 +42,15 @@ __global__ void pack_mlp_kernel(const float* __restrict__ mlp, unsigned char* __
   }
 }
 
+// fp32 accumulator tile [128][SCR_LD] (<= 64 columns + 8 of padding: conflict-free fragment stores)
+constexpr int SCR_LD = 72;
+constexpr int SCR_BYTES = 128 * SCR_LD * 4;
+
 struct FwdSmem {
   static constexpr int W = 0;                 // PW_TOTAL (1024-aligned images)
   static constexpr int A = 28672;             // [128][128 B]
-  static constexpr int BAR = A + 16384;
+  static constexpr int SCR = A + 16384;       // accumulator tile
+  static constexpr int BAR = SCR + SCR_BYTES;
   static constexpr int TOTAL = BAR + 64;
 };
 
@@ -56,17 +61,30 @@ __device__ __forceinline__ void store_row_chunk(unsigned char* arow, int row, in
   *reinterpret_cast<uint4*>(arow + ((chunk ^ (row & 7)) << 4)) = *reinterpret_cast<const uint4*>(h2);
 }
 
-// one layer: A tile (already written + fenced + synced) x packed weights -> TMEM cols [0,N)
+// one layer, issued by the whole CTA (one warpgroup): A tile (already written + fenced + synced, 128 rows) x packed
+// weights -> fp32 tile scr[128][SCR_LD] columns [0, N), visible to every thread on return
 template <int N>
-// called by the WHOLE warp 0 (uniform control flow), issued by its elected lane (`lead`): see tc::umma_f16_lead
-__device__ __forceinline__ void issue_layer(uint32_t a_addr, uint32_t b_addr, uint32_t tmem, int ksteps, uint64_t* bar,
-                                            uint32_t lead) {
-  constexpr uint32_t idesc = tc::umma_idesc_f16(128, N, 0);
-  tc::tc_fence_after();
-  const uint64_t ad = tc::umma_desc_sw128(a_addr), bd = tc::umma_desc_sw128(b_addr);
-  for (int k = 0; k < ksteps; k++)
-    tc::umma_f16_lead(tmem, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), idesc, k ? 1u : 0u, lead);
-  tc::umma_commit_lead(bar, lead);
+__device__ __forceinline__ void mma_layer(uint32_t a_addr, uint32_t b_addr, int ksteps, float* scr, int tid) {
+  float d[2][N / 2];
+#pragma unroll
+  for (int h = 0; h < 2; h++)
+#pragma unroll
+    for (int i = 0; i < N / 2; i++) d[h][i] = 0.f;
+  const uint64_t bd = tc::desc_sw128(b_addr);
+  tc::wgmma_fence();
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    const uint64_t ad = tc::desc_sw128(a_addr + h * 8192);      // rows 64h .. 64h+63
+    for (int k = 0; k < ksteps; k++) tc::wgmma_f16<N>(d[h], ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), k ? 1u : 0u);
+  }
+  tc::wgmma_commit();
+  tc::wgmma_wait<0>();
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    tc::acc_fence(d[h]);
+    tc::acc_to_smem<N>(scr, SCR_LD, 64 * h, 0, d[h], tid);
+  }
+  __syncthreads();
 }
 
 __global__ void __launch_bounds__(128)
@@ -75,27 +93,18 @@ forward_tc_kernel(const float* __restrict__ coords, const int* __restrict__ coun
                   float* __restrict__ rgbsigma, __half* __restrict__ enc_out) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* bar = reinterpret_cast<uint64_t*>(sm + FwdSmem::BAR);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar + 1);
-  const int tid = threadIdx.x, warp = tid >> 5;
+  float* scr = reinterpret_cast<float*>(sm + FwdSmem::SCR);
+  const int tid = threadIdx.x;
   const int n = n_fixed >= 0 ? n_fixed : counters[0];
   const int ntiles = (n + 127) / 128;
 
   for (int i = tid; i < PW_TOTAL / 16; i += 128)
     reinterpret_cast<uint4*>(sm + FwdSmem::W)[i] = reinterpret_cast<const uint4*>(packed)[i];
-  if (tid == 0) { tc::mbar_init(bar, 1); tc::fence_barrier_init(); }
-  const uint32_t lead = (tid < 32) ? (tc::elect_one() ? 1u : 0u) : 0u;      // MMA-issuing lane of warp 0
-  if (warp == 0) tc::tmem_alloc<64>(tmem_slot);
   tc::fence_proxy_async();
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16);
   const uint32_t a_addr = tc::smem_u32(sm + FwdSmem::A);
   const uint32_t w_addr = tc::smem_u32(sm + FwdSmem::W);
   unsigned char* arow = sm + FwdSmem::A + tid * 128;
-  uint32_t phase = 0;
 
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const int s = tile * 128 + tid;
@@ -122,19 +131,15 @@ forward_tc_kernel(const float* __restrict__ coords, const int* __restrict__ coun
       }
     }
     tc::fence_proxy_async();
-    tc::tc_fence_before();
     __syncthreads();
     // ---- layer 1: 32 -> 64, ReLU
-    if (tid < 32) issue_layer<64>(a_addr, w_addr + PW1, tmem, 2, bar, lead);
-    tc::mbar_wait(bar, phase & 1); phase++;
-    tc::tc_fence_after();
+    mma_layer<64>(a_addr, w_addr + PW1, 2, scr, tid);
     {
       uint32_t r[32];
       float v[8];
 #pragma unroll
       for (int h = 0; h < 2; h++) {
-        tc::tmem_ld_32x32(taddr + h * 32, r);
-        tc::tmem_ld_wait();
+        tc::smem_row_ld<32>(scr, SCR_LD, tid, h * 32, r);
 #pragma unroll
         for (int c = 0; c < 4; c++) {
 #pragma unroll
@@ -144,17 +149,13 @@ forward_tc_kernel(const float* __restrict__ coords, const int* __restrict__ coun
       }
     }
     tc::fence_proxy_async();
-    tc::tc_fence_before();
     __syncthreads();
     // ---- layer 2: 64 -> 16 (density head)
-    if (tid < 32) issue_layer<16>(a_addr, w_addr + PW2, tmem, 4, bar, lead);
-    tc::mbar_wait(bar, phase & 1); phase++;
-    tc::tc_fence_after();
+    mma_layer<16>(a_addr, w_addr + PW2, 4, scr, tid);
     float sigma;
     {
       uint32_t r[32];
-      tc::tmem_ld_32x32(taddr, r);     // 16 valid columns
-      tc::tmem_ld_wait();
+      tc::smem_row_ld<32>(scr, SCR_LD, tid, 0, r);     // 16 valid columns
       float o[16], sh[16];
 #pragma unroll
       for (int j = 0; j < 16; j++) o[j] = __uint_as_float(r[j]);
@@ -167,20 +168,16 @@ forward_tc_kernel(const float* __restrict__ coords, const int* __restrict__ coun
       for (int c = 4; c < 8; c++) store_row_chunk(arow, tid, c, z8);
     }
     tc::fence_proxy_async();
-    tc::tc_fence_before();
     __syncthreads();
     // ---- layers 3, 4: -> 64, ReLU
 #pragma unroll 1
     for (int l = 0; l < 2; l++) {
-      if (tid < 32) issue_layer<64>(a_addr, w_addr + (l == 0 ? PW3 : PW4), tmem, l == 0 ? 2 : 4, bar, lead);
-      tc::mbar_wait(bar, phase & 1); phase++;
-      tc::tc_fence_after();
+      mma_layer<64>(a_addr, w_addr + (l == 0 ? PW3 : PW4), l == 0 ? 2 : 4, scr, tid);
       uint32_t r[32];
       float v[8];
 #pragma unroll
       for (int h = 0; h < 2; h++) {
-        tc::tmem_ld_32x32(taddr + h * 32, r);
-        tc::tmem_ld_wait();
+        tc::smem_row_ld<32>(scr, SCR_LD, tid, h * 32, r);
 #pragma unroll
         for (int c = 0; c < 4; c++) {
 #pragma unroll
@@ -189,17 +186,13 @@ forward_tc_kernel(const float* __restrict__ coords, const int* __restrict__ coun
         }
       }
       tc::fence_proxy_async();
-      tc::tc_fence_before();
       __syncthreads();
     }
     // ---- layer 5: 64 -> 3 (16), sigmoid
-    if (tid < 32) issue_layer<16>(a_addr, w_addr + PW5, tmem, 4, bar, lead);
-    tc::mbar_wait(bar, phase & 1); phase++;
-    tc::tc_fence_after();
+    mma_layer<16>(a_addr, w_addr + PW5, 4, scr, tid);
     {
       uint32_t r[32];
-      tc::tmem_ld_32x32(taddr, r);
-      tc::tmem_ld_wait();
+      tc::smem_row_ld<32>(scr, SCR_LD, tid, 0, r);
       if (act) {
         float4 out;
         out.x = 1.f / (1.f + __expf(-__uint_as_float(r[0])));
@@ -209,12 +202,8 @@ forward_tc_kernel(const float* __restrict__ coords, const int* __restrict__ coun
         reinterpret_cast<float4*>(rgbsigma)[s] = out;
       }
     }
-    tc::tc_fence_before();
-    __syncthreads();      // TMEM + A tile reusable by the next tile
+    __syncthreads();      // accumulator tile + A tile reusable by the next tile
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<64>(tmem);
 }
 
 
@@ -222,13 +211,12 @@ forward_tc_kernel(const float* __restrict__ coords, const int* __restrict__ coun
 // Backward on tensor cores.  Per 128-sample tile (thread = sample):
 //   forward recompute (layers 1-4) keeping every layer's INPUT tile in shared memory,
 //   then for l = 5..1 two MMA groups per layer, issued together:
-//     dW_l   += A_l^T (features x samples) . delta_l (samples x N_l)     [accumulates in TMEM across tiles]
+//     dW_l   += A_l^T (features x samples) . delta_l (samples x N_l)     [M = 64 features; fp32 fragments
+//                                                                         accumulate in registers across tiles]
 //     dIn_l   = delta_l (samples x N_l)    . W_l^T                       [-> ACC, masked by ReLU']
 //   Operands are fp16 (deltas carry a loss scale), accumulation fp32.  The transposed operand
 //   tiles (K = the 128 samples) are written by the owning threads with 2-byte swizzled stores.
 //   At the end of the persistent loop each CTA flushes its dW accumulators with fp32 atomics.
-// TMEM (512 columns): ACC [0,64) | dW1 [64,128) | dW2 [128,144) | dW3 [160,224) | dW4 [224,288) | dW5 [288,304)
-constexpr int TM_ACC = 0, TM_DW1 = 64, TM_DW2 = 128, TM_DW3 = 160, TM_DW4 = 224, TM_DW5 = 288;
 // backward weight images B[k][n] = W[k][n], n padded to 64: WB5 [64][128B], WB4 [64][128B], WB3 [32][128B], WB2 [64][128B], WB1 [32][128B]
 constexpr int PB5 = 0, PB4 = 8192, PB3 = 16384, PB2 = 20480, PB1 = 28672, PB_TOTAL = 32768;
 
@@ -256,11 +244,13 @@ struct BwdSmem {
   static constexpr int W = 0;                      // forward images   28672
   static constexpr int WB = 28672;                 // backward images  32768
   static constexpr int ACT = WB + PB_TOTAL;        // 5 x 16384 : inputs of layers 1..5 (row-major, swizzled)
-  static constexpr int AT = ACT + 5 * 16384;       // transposed activations: 2 halves x [128][128B]
-  static constexpr int D = AT + 32768;             // delta, row-major [128][128B]
+  static constexpr int AT = ACT + 5 * 16384;       // transposed activations: 2 sample halves x [64 features][128B]
+  static constexpr int D = AT + 16384;             // delta, row-major [128][128B]
   static constexpr int DT = D + 16384;             // delta transposed: 2 halves x [64][128B]
-  static constexpr int BAR = DT + 16384;
+  static constexpr int SCR = DT + 16384;           // fp32 accumulator tile [128][SCR_LD]
+  static constexpr int BAR = SCR + SCR_BYTES;
   static constexpr int TOTAL = BAR + 64;
+  static_assert(TOTAL + 1024 <= 227 * 1024, "shared memory plan");
 };
 
 // element (row f, sample s) of a K-major [rows][128 samples] operand split in two 64-sample halves
@@ -277,7 +267,7 @@ __device__ __forceinline__ void transpose_row(const unsigned char* tile, unsigne
 #pragma unroll
     for (int j = 0; j < 8; j++) {
       const int f = c * 8 + j;
-      __half* p = reinterpret_cast<__half*>(at + (row >> 6) * 16384 + f * 128 + ((((row & 63) >> 3) ^ (f & 7)) << 4)) + (row & 7);
+      __half* p = reinterpret_cast<__half*>(at + (row >> 6) * 8192 + f * 128 + ((((row & 63) >> 3) ^ (f & 7)) << 4)) + (row & 7);
       *p = h[j];
     }
   }
@@ -293,32 +283,59 @@ __device__ __forceinline__ void store_delta(unsigned char* dtile, unsigned char*
   for (int n = 0; n < NV; n++) store_T(dt, 8192, n, row, d[n]);
 }
 
-// dW (TMEM cols at `tm_dw`, N columns) += AT^T-operand x DT-operand over the 128 samples; then
-// ACC = D x WB (N_out columns, `ks` K-steps).  Issued by one thread; one commit covers both.
+// dW (fragments `dw`, M = 64 features x N) += AT-operand x DT-operand over the 128 samples; then
+// scr = D x WB (N_out columns, `ks` K-steps).  Issued by the whole CTA (one warpgroup), one commit covers both.
 template <int N, int NOUT>
-__device__ __forceinline__ void issue_bwd_layer(uint32_t at_addr, uint32_t dt_addr, uint32_t d_addr, uint32_t wb_addr,
-                                                uint32_t tmem, int tm_dw, int ks, bool first_tile, uint64_t* bar, uint32_t lead) {
-  constexpr uint32_t idw = tc::umma_idesc_f16(128, N, 0);
-  constexpr uint32_t idp = tc::umma_idesc_f16(128, NOUT, 0);
-  tc::tc_fence_after();
+__device__ __forceinline__ void mma_bwd_layer(uint32_t at_addr, uint32_t dt_addr, uint32_t d_addr, uint32_t wb_addr,
+                                              float (&dw)[N / 2], int ks, float* scr, int tid) {
+  float acc[2][NOUT / 2];
+#pragma unroll
+  for (int h = 0; h < 2; h++)
+#pragma unroll
+    for (int i = 0; i < NOUT / 2; i++) acc[h][i] = 0.f;
+  tc::wgmma_fence();
+  tc::acc_fence(dw);
 #pragma unroll
   for (int h = 0; h < 2; h++)
 #pragma unroll
     for (int k = 0; k < 4; k++)
-      tc::umma_f16_lead(tmem + tm_dw, tc::umma_desc_sw128(at_addr + h * 16384 + k * 32),
-                        tc::umma_desc_sw128(dt_addr + h * 8192 + k * 32), idw, (first_tile && h == 0 && k == 0) ? 0u : 1u, lead);
-  for (int k = 0; k < ks; k++)
-    tc::umma_f16_lead(tmem + TM_ACC, tc::umma_desc_sw128(d_addr + k * 32), tc::umma_desc_sw128(wb_addr + k * 32), idp, k ? 1u : 0u, lead);
-  tc::umma_commit_lead(bar, lead);
+      tc::wgmma_f16<N>(dw, tc::desc_sw128(at_addr + h * 8192 + k * 32), tc::desc_sw128(dt_addr + h * 8192 + k * 32), 1u);
+  const uint64_t bd = tc::desc_sw128(wb_addr);
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    const uint64_t ad = tc::desc_sw128(d_addr + h * 8192);
+    for (int k = 0; k < ks; k++) tc::wgmma_f16<NOUT>(acc[h], ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), k ? 1u : 0u);
+  }
+  tc::wgmma_commit();
+  tc::wgmma_wait<0>();
+  tc::acc_fence(dw);
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    tc::acc_fence(acc[h]);
+    tc::acc_to_smem<NOUT>(scr, SCR_LD, 64 * h, 0, acc[h], tid);
+  }
+  __syncthreads();
 }
 
-__device__ __forceinline__ void ld_relu_store(uint32_t taddr, unsigned char* arow, int row, uint32_t* mask) {
+// weight-gradient flush: fragment element (feature k, column n) of dW [kmax][N] -> this CTA's slot of the partials
+template <int N>
+__device__ __forceinline__ void flush_dw(const float (&d)[N / 2], float* __restrict__ g, int kmax, float scale, int tid) {
+  const int w = tid >> 5, l = tid & 31;
+#pragma unroll
+  for (int j = 0; j < N / 8; j++)
+#pragma unroll
+    for (int i = 0; i < 2; i++) {
+      const int k = 16 * w + (l >> 2) + 8 * i, n = 8 * j + 2 * (l & 3);
+      if (k < kmax) *reinterpret_cast<float2*>(g + k * N + n) = make_float2(d[4 * j + 2 * i] * scale, d[4 * j + 2 * i + 1] * scale);
+    }
+}
+
+__device__ __forceinline__ void ld_relu_store(const float* scr, unsigned char* arow, int row, uint32_t* mask) {
   uint32_t r[32];
   float v[8];
 #pragma unroll
   for (int h = 0; h < 2; h++) {
-    tc::tmem_ld_32x32(taddr + h * 32, r);
-    tc::tmem_ld_wait();
+    tc::smem_row_ld<32>(scr, SCR_LD, row, h * 32, r);
     uint32_t m = 0;
 #pragma unroll
     for (int c = 0; c < 4; c++) {
@@ -337,7 +354,6 @@ __device__ __forceinline__ void ld_relu_store(uint32_t taddr, unsigned char* aro
 #define NGP_TC_SYNC()            \
   do {                           \
     tc::fence_proxy_async();     \
-    tc::tc_fence_before();       \
     __syncthreads();             \
   } while (0)
 
@@ -345,25 +361,18 @@ __global__ void __launch_bounds__(128, 1)
 backward_tc_kernel(const float* __restrict__ coords, const int* __restrict__ counters,
                    const __half2* __restrict__ grid, LevelInfo lv, const unsigned char* __restrict__ packed_fwd,
                    const unsigned char* __restrict__ packed_bwd, const float* __restrict__ dout,
-                   float* __restrict__ mlp_grad, float* __restrict__ grid_grad, float loss_scale,
+                   float* __restrict__ dw_part, float* __restrict__ grid_grad, float loss_scale,
                    const __half* __restrict__ enc_in, __half* __restrict__ denc_out) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* bar = reinterpret_cast<uint64_t*>(sm + BwdSmem::BAR);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar + 1);
-  const int tid = threadIdx.x, warp = tid >> 5;
+  float* scr = reinterpret_cast<float*>(sm + BwdSmem::SCR);
+  const int tid = threadIdx.x;
   const int n = counters[0];
   const int ntiles = (n + 127) / 128;
   for (int i = tid; i < PW_TOTAL / 16; i += 128) reinterpret_cast<uint4*>(sm + BwdSmem::W)[i] = reinterpret_cast<const uint4*>(packed_fwd)[i];
   for (int i = tid; i < PB_TOTAL / 16; i += 128) reinterpret_cast<uint4*>(sm + BwdSmem::WB)[i] = reinterpret_cast<const uint4*>(packed_bwd)[i];
-  for (int i = tid; i < (32768 + 16384 + 16384) / 16; i += 128) reinterpret_cast<uint4*>(sm + BwdSmem::AT)[i] = make_uint4(0, 0, 0, 0);
-  if (tid == 0) { tc::mbar_init(bar, 1); tc::fence_barrier_init(); }
-  const uint32_t lead = (tid < 32) ? (tc::elect_one() ? 1u : 0u) : 0u;      // MMA-issuing lane of warp 0
-  if (warp == 0) tc::tmem_alloc<512>(tmem_slot);
+  for (int i = tid; i < (16384 + 16384 + 16384) / 16; i += 128) reinterpret_cast<uint4*>(sm + BwdSmem::AT)[i] = make_uint4(0, 0, 0, 0);
   NGP_TC_SYNC();
-  tc::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16);
   const uint32_t w_addr = tc::smem_u32(sm + BwdSmem::W), wb_addr = tc::smem_u32(sm + BwdSmem::WB);
   const uint32_t act_addr = tc::smem_u32(sm + BwdSmem::ACT);
   const uint32_t at_addr = tc::smem_u32(sm + BwdSmem::AT), d_addr = tc::smem_u32(sm + BwdSmem::D), dt_addr = tc::smem_u32(sm + BwdSmem::DT);
@@ -371,9 +380,14 @@ backward_tc_kernel(const float* __restrict__ coords, const int* __restrict__ cou
   unsigned char* AT = sm + BwdSmem::AT;
   unsigned char* Dt = sm + BwdSmem::D;
   unsigned char* DT = sm + BwdSmem::DT;
-  uint32_t phase = 0;
   bool first = true;
   const float inv_scale = 1.f / loss_scale;
+  // weight-gradient accumulators (rows = input features 0..63)
+  float dw1[32], dw2[8], dw3[32], dw4[32], dw5[8];
+#pragma unroll
+  for (int i = 0; i < 32; i++) { dw1[i] = 0.f; dw3[i] = 0.f; dw4[i] = 0.f; }
+#pragma unroll
+  for (int i = 0; i < 8; i++) { dw2[i] = 0.f; dw5[i] = 0.f; }
 
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const int s = tile * 128 + tid;
@@ -409,18 +423,13 @@ backward_tc_kernel(const float* __restrict__ coords, const int* __restrict__ cou
       for (int c = 4; c < 8; c++) store_row_chunk(a0, tid, c, z8);
     }
     NGP_TC_SYNC();
-    if (tid < 32) issue_layer<64>(act_addr + 0 * 16384, w_addr + PW1, tmem + TM_ACC, 2, bar, lead);
-    tc::mbar_wait(bar, phase & 1); phase++;
-    tc::tc_fence_after();
-    ld_relu_store(taddr + TM_ACC, act + 1 * 16384 + tid * 128, tid, m1);
+    mma_layer<64>(act_addr + 0 * 16384, w_addr + PW1, 2, scr, tid);
+    ld_relu_store(scr, act + 1 * 16384 + tid * 128, tid, m1);
     NGP_TC_SYNC();
-    if (tid < 32) issue_layer<16>(act_addr + 1 * 16384, w_addr + PW2, tmem + TM_ACC, 4, bar, lead);
-    tc::mbar_wait(bar, phase & 1); phase++;
-    tc::tc_fence_after();
+    mma_layer<16>(act_addr + 1 * 16384, w_addr + PW2, 4, scr, tid);
     {
       uint32_t r[32];
-      tc::tmem_ld_32x32(taddr + TM_ACC, r);
-      tc::tmem_ld_wait();
+      tc::smem_row_ld<32>(scr, SCR_LD, tid, 0, r);
       float o[16], sh[16];
 #pragma unroll
       for (int j = 0; j < 16; j++) o[j] = __uint_as_float(r[j]);
@@ -433,15 +442,11 @@ backward_tc_kernel(const float* __restrict__ coords, const int* __restrict__ cou
       for (int c = 4; c < 8; c++) store_row_chunk(a2, tid, c, z8);
     }
     NGP_TC_SYNC();
-    if (tid < 32) issue_layer<64>(act_addr + 2 * 16384, w_addr + PW3, tmem + TM_ACC, 2, bar, lead);
-    tc::mbar_wait(bar, phase & 1); phase++;
-    tc::tc_fence_after();
-    ld_relu_store(taddr + TM_ACC, act + 3 * 16384 + tid * 128, tid, m3);
+    mma_layer<64>(act_addr + 2 * 16384, w_addr + PW3, 2, scr, tid);
+    ld_relu_store(scr, act + 3 * 16384 + tid * 128, tid, m3);
     NGP_TC_SYNC();
-    if (tid < 32) issue_layer<64>(act_addr + 3 * 16384, w_addr + PW4, tmem + TM_ACC, 4, bar, lead);
-    tc::mbar_wait(bar, phase & 1); phase++;
-    tc::tc_fence_after();
-    ld_relu_store(taddr + TM_ACC, act + 4 * 16384 + tid * 128, tid, m4);
+    mma_layer<64>(act_addr + 3 * 16384, w_addr + PW4, 4, scr, tid);
+    ld_relu_store(scr, act + 4 * 16384 + tid * 128, tid, m4);
     // ---------------- layer 5 backward: delta5 = d(raw rgb)
     float d64[64];
     {
@@ -451,88 +456,69 @@ backward_tc_kernel(const float* __restrict__ coords, const int* __restrict__ cou
     __syncthreads();                                   // ACT4 rows complete before anyone transposes... (own row only) 
     transpose_row(act + 4 * 16384, AT, tid, 64);
     NGP_TC_SYNC();
-    if (tid < 32) issue_bwd_layer<16, 64>(at_addr, dt_addr, d_addr, wb_addr + PB5, tmem, TM_DW5, 1, first, bar, lead);
-    tc::mbar_wait(bar, phase & 1); phase++;
-    tc::tc_fence_after();
+    mma_bwd_layer<16, 64>(at_addr, dt_addr, d_addr, wb_addr + PB5, dw5, 1, scr, tid);
     {
       uint32_t r[32];
 #pragma unroll
       for (int h = 0; h < 2; h++) {
-        tc::tmem_ld_32x32(taddr + TM_ACC + h * 32, r);
-        tc::tmem_ld_wait();
+        tc::smem_row_ld<32>(scr, SCR_LD, tid, h * 32, r);
 #pragma unroll
         for (int j = 0; j < 32; j++) d64[h * 32 + j] = ((m4[h] >> j) & 1u) ? __uint_as_float(r[j]) : 0.f;
       }
     }
-    tc::tc_fence_before();
     __syncthreads();
     // ---------------- layer 4
     store_delta<64>(Dt, DT, tid, d64);
     transpose_row(act + 3 * 16384, AT, tid, 64);
     NGP_TC_SYNC();
-    if (tid < 32) issue_bwd_layer<64, 64>(at_addr, dt_addr, d_addr, wb_addr + PB4, tmem, TM_DW4, 4, first, bar, lead);
-    tc::mbar_wait(bar, phase & 1); phase++;
-    tc::tc_fence_after();
+    mma_bwd_layer<64, 64>(at_addr, dt_addr, d_addr, wb_addr + PB4, dw4, 4, scr, tid);
     {
       uint32_t r[32];
 #pragma unroll
       for (int h = 0; h < 2; h++) {
-        tc::tmem_ld_32x32(taddr + TM_ACC + h * 32, r);
-        tc::tmem_ld_wait();
+        tc::smem_row_ld<32>(scr, SCR_LD, tid, h * 32, r);
 #pragma unroll
         for (int j = 0; j < 32; j++) d64[h * 32 + j] = ((m3[h] >> j) & 1u) ? __uint_as_float(r[j]) : 0.f;
       }
     }
-    tc::tc_fence_before();
     __syncthreads();
     // ---------------- layer 3 (input = [o(16) | sh(16)])
     store_delta<64>(Dt, DT, tid, d64);
     transpose_row(act + 2 * 16384, AT, tid, 32);
     NGP_TC_SYNC();
-    if (tid < 32) issue_bwd_layer<64, 32>(at_addr, dt_addr, d_addr, wb_addr + PB3, tmem, TM_DW3, 4, first, bar, lead);
-    tc::mbar_wait(bar, phase & 1); phase++;
-    tc::tc_fence_after();
+    mma_bwd_layer<64, 32>(at_addr, dt_addr, d_addr, wb_addr + PB3, dw3, 4, scr, tid);
     float d16[16];
     {
       uint32_t r[32];
-      tc::tmem_ld_32x32(taddr + TM_ACC, r);
-      tc::tmem_ld_wait();
+      tc::smem_row_ld<32>(scr, SCR_LD, tid, 0, r);
 #pragma unroll
       for (int j = 0; j < 16; j++) d16[j] = __uint_as_float(r[j]);
       d16[0] += dg.w;                                   // sigma path: d/d o0
     }
-    tc::tc_fence_before();
     __syncthreads();
     // ---------------- layer 2
     store_delta<16>(Dt, DT, tid, d16);
     transpose_row(act + 1 * 16384, AT, tid, 64);
     NGP_TC_SYNC();
-    if (tid < 32) issue_bwd_layer<16, 64>(at_addr, dt_addr, d_addr, wb_addr + PB2, tmem, TM_DW2, 1, first, bar, lead);
-    tc::mbar_wait(bar, phase & 1); phase++;
-    tc::tc_fence_after();
+    mma_bwd_layer<16, 64>(at_addr, dt_addr, d_addr, wb_addr + PB2, dw2, 1, scr, tid);
     {
       uint32_t r[32];
 #pragma unroll
       for (int h = 0; h < 2; h++) {
-        tc::tmem_ld_32x32(taddr + TM_ACC + h * 32, r);
-        tc::tmem_ld_wait();
+        tc::smem_row_ld<32>(scr, SCR_LD, tid, h * 32, r);
 #pragma unroll
         for (int j = 0; j < 32; j++) d64[h * 32 + j] = ((m1[h] >> j) & 1u) ? __uint_as_float(r[j]) : 0.f;
       }
     }
-    tc::tc_fence_before();
     __syncthreads();
     // ---------------- layer 1
     store_delta<64>(Dt, DT, tid, d64);
     transpose_row(act + 0 * 16384, AT, tid, 32);
     NGP_TC_SYNC();
-    if (tid < 32) issue_bwd_layer<64, 32>(at_addr, dt_addr, d_addr, wb_addr + PB1, tmem, TM_DW1, 4, first, bar, lead);
-    tc::mbar_wait(bar, phase & 1); phase++;
-    tc::tc_fence_after();
+    mma_bwd_layer<64, 32>(at_addr, dt_addr, d_addr, wb_addr + PB1, dw1, 4, scr, tid);
     {
       uint32_t r[32];
-      tc::tmem_ld_32x32(taddr + TM_ACC, r);             // d/d enc [32], still loss-scaled
-      tc::tmem_ld_wait();
+      tc::smem_row_ld<32>(scr, SCR_LD, tid, 0, r);             // d/d enc [32], still loss-scaled
       if (denc_out) {
         // hand the (loss-scaled, fp16) encoding gradient to the scatter kernel
         if (actv) {
@@ -564,36 +550,26 @@ backward_tc_kernel(const float* __restrict__ coords, const int* __restrict__ cou
         }
       }
     }
-    tc::tc_fence_before();
     __syncthreads();
     first = false;
   }
-  // ---------------- flush the weight-gradient accumulators (row = input feature k = TMEM lane)
-  if (!first) {
-    tc::tc_fence_after();
-    const int k = tid;
-    uint32_t r[32];
-    // dW1 [32][64]
-    for (int h = 0; h < 2; h++) {
-      tc::tmem_ld_32x32(taddr + TM_DW1 + h * 32, r); tc::tmem_ld_wait();
-      if (k < 32) for (int j = 0; j < 32; j++) atomicAdd(mlp_grad + W1_OFF + k * 64 + h * 32 + j, __uint_as_float(r[j]) * inv_scale);
-    }
-    tc::tmem_ld_32x32(taddr + TM_DW2, r); tc::tmem_ld_wait();
-    if (k < 64) for (int j = 0; j < 16; j++) atomicAdd(mlp_grad + W2_OFF + k * 16 + j, __uint_as_float(r[j]) * inv_scale);
-    for (int h = 0; h < 2; h++) {
-      tc::tmem_ld_32x32(taddr + TM_DW3 + h * 32, r); tc::tmem_ld_wait();
-      if (k < 32) for (int j = 0; j < 32; j++) atomicAdd(mlp_grad + W3_OFF + k * 64 + h * 32 + j, __uint_as_float(r[j]) * inv_scale);
-    }
-    for (int h = 0; h < 2; h++) {
-      tc::tmem_ld_32x32(taddr + TM_DW4 + h * 32, r); tc::tmem_ld_wait();
-      if (k < 64) for (int j = 0; j < 32; j++) atomicAdd(mlp_grad + W4_OFF + k * 64 + h * 32 + j, __uint_as_float(r[j]) * inv_scale);
-    }
-    tc::tmem_ld_32x32(taddr + TM_DW5, r); tc::tmem_ld_wait();
-    if (k < 64) for (int j = 0; j < 16; j++) atomicAdd(mlp_grad + W5_OFF + k * 16 + j, __uint_as_float(r[j]) * inv_scale);
-  }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<512>(tmem);
+  // ---------------- flush the weight-gradient accumulators into this CTA's slot (zeros when it had no tile);
+  // dw_reduce_kernel adds the slots in CTA order
+  float* g = dw_part + (size_t)blockIdx.x * W_TOTAL;
+  flush_dw<64>(dw1, g + W1_OFF, 32, inv_scale, tid);
+  flush_dw<16>(dw2, g + W2_OFF, 64, inv_scale, tid);
+  flush_dw<64>(dw3, g + W3_OFF, 32, inv_scale, tid);
+  flush_dw<64>(dw4, g + W4_OFF, 64, inv_scale, tid);
+  flush_dw<16>(dw5, g + W5_OFF, 64, inv_scale, tid);
+}
+
+// mlp_grad[i] += sum over CTAs c (in order) of dw_part[c][i]
+__global__ void dw_reduce_kernel(const float* __restrict__ dw_part, int nparts, float* __restrict__ mlp_grad) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= W_TOTAL) return;
+  float s = 0.f;
+  for (int c = 0; c < nparts; c++) s += dw_part[(size_t)c * W_TOTAL + i];
+  mlp_grad[i] += s;
 }
 
 
@@ -603,9 +579,11 @@ backward_tc_kernel(const float* __restrict__ coords, const int* __restrict__ cou
 // cell on the coarse levels (cell >> step), so equal table indices form runs across the lanes; each
 // run is summed with a segmented shuffle scan and only its head lane issues the atomic (about 40 %
 // fewer atomics overall, >90 % fewer on the contended coarse levels).
+constexpr float GRID_FX = 1099511627776.f;          // 2^40: fixed-point scale of the hash-grid gradient accumulator
+
 __global__ void __launch_bounds__(256)
 grid_scatter_kernel(const float* __restrict__ coords, const int* __restrict__ counters, const __half* __restrict__ denc,
-                    LevelInfo lv, float* __restrict__ grid_grad, float inv_scale) {
+                    LevelInfo lv, long long* __restrict__ grid_acc, float inv_scale) {
   const int n = counters[0];
   const int lane = threadIdx.x & 31;
   const size_t nwork = ((size_t)(n + 31) / 32) * N_LEVELS;              // (32-sample group, level) per warp
@@ -625,7 +603,7 @@ grid_scatter_kernel(const float* __restrict__ coords, const int* __restrict__ co
       wx = px - fx; wy = py - fy; wz = pz - fz;
       ix = (int)fx; iy = (int)fy; iz = (int)fz;
     }
-    float2* gg = reinterpret_cast<float2*>(grid_grad) + lv.offset[l];
+    long long* gg = grid_acc + 2 * (size_t)lv.offset[l];
 #pragma unroll
     for (int c = 0; c < 8; c++) {
       const int dx = c & 1, dy = (c >> 1) & 1, dz = c >> 2;
@@ -643,7 +621,7 @@ grid_scatter_kernel(const float* __restrict__ coords, const int* __restrict__ co
         const float na = __shfl_down_sync(0xffffffffu, va, o), nb = __shfl_down_sync(0xffffffffu, vb, o);
         if (lane + o < 32 && nr == run) { va += na; vb += nb; }
       }
-      if (head && actv && (va != 0.f || vb != 0.f)) atomicAdd(gg + idx, make_float2(va, vb));
+      if (head && actv && (va != 0.f || vb != 0.f)) { fx_add(gg + 2 * (size_t)idx, va, GRID_FX); fx_add(gg + 2 * (size_t)idx + 1, vb, GRID_FX); }
     }
   }
 }
@@ -656,24 +634,16 @@ density_tc_kernel(const __half2* __restrict__ grid, LevelInfo lv, const unsigned
                   float* __restrict__ density) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* bar = reinterpret_cast<uint64_t*>(sm + FwdSmem::BAR);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar + 1);
-  const int tid = threadIdx.x, warp = tid >> 5;
+  float* scr = reinterpret_cast<float*>(sm + FwdSmem::SCR);
+  const int tid = threadIdx.x;
   const int total = n_per_cascade * cascades;
   const int ntiles = (total + 127) / 128;
   for (int i = tid; i < PW3 / 16; i += 128)          // W1 and W2 images only
     reinterpret_cast<uint4*>(sm + FwdSmem::W)[i] = reinterpret_cast<const uint4*>(packed)[i];
-  if (tid == 0) { tc::mbar_init(bar, 1); tc::fence_barrier_init(); }
-  const uint32_t lead = (tid < 32) ? (tc::elect_one() ? 1u : 0u) : 0u;      // MMA-issuing lane of warp 0
-  if (warp == 0) tc::tmem_alloc<64>(tmem_slot);
   NGP_TC_SYNC();
-  tc::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16);
   const uint32_t a_addr = tc::smem_u32(sm + FwdSmem::A), w_addr = tc::smem_u32(sm + FwdSmem::W);
   unsigned char* arow = sm + FwdSmem::A + tid * 128;
   const int NC = GRID * GRID * GRID;
-  uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const int i = tile * 128 + tid;
     bool actv = i < total;
@@ -681,7 +651,7 @@ density_tc_kernel(const __half2* __restrict__ grid, LevelInfo lv, const unsigned
     float s = 1.f, x01[3] = {0.5f, 0.5f, 0.5f};
     if (actv) {
       const int mip = i / n_per_cascade, j = i % n_per_cascade;
-      const uint32_t cell = (n_per_cascade >= NC) ? (uint32_t)j : (pcg(pcg(seed) ^ (uint32_t)i) % NC);
+      const uint32_t cell = (n_per_cascade >= NC) ? (uint32_t)j : density_cell(seed, mip, j);
       gi = (size_t)mip * NC + cell;
       actv = density[gi] >= 0.f;                     // never visible from a training camera -> skip
       const int ix = cell % GRID, iy = (cell / GRID) % GRID, iz = cell / (GRID * GRID);
@@ -707,16 +677,13 @@ density_tc_kernel(const __half2* __restrict__ grid, LevelInfo lv, const unsigned
       for (int c = 4; c < 8; c++) store_row_chunk(arow, tid, c, z8);
     }
     NGP_TC_SYNC();
-    if (tid < 32) issue_layer<64>(a_addr, w_addr + PW1, tmem, 2, bar, lead);
-    tc::mbar_wait(bar, phase & 1); phase++;
-    tc::tc_fence_after();
+    mma_layer<64>(a_addr, w_addr + PW1, 2, scr, tid);
     {
       uint32_t r[32];
       float v[8];
 #pragma unroll
       for (int h = 0; h < 2; h++) {
-        tc::tmem_ld_32x32(taddr + h * 32, r);
-        tc::tmem_ld_wait();
+        tc::smem_row_ld<32>(scr, SCR_LD, tid, h * 32, r);
 #pragma unroll
         for (int c = 0; c < 4; c++) {
 #pragma unroll
@@ -726,24 +693,17 @@ density_tc_kernel(const __half2* __restrict__ grid, LevelInfo lv, const unsigned
       }
     }
     NGP_TC_SYNC();
-    if (tid < 32) issue_layer<16>(a_addr, w_addr + PW2, tmem, 4, bar, lead);
-    tc::mbar_wait(bar, phase & 1); phase++;
-    tc::tc_fence_after();
+    mma_layer<16>(a_addr, w_addr + PW2, 4, scr, tid);
     {
       uint32_t r[32];
-      tc::tmem_ld_32x32(taddr, r);
-      tc::tmem_ld_wait();
+      tc::smem_row_ld<32>(scr, SCR_LD, tid, 0, r);
       if (actv) {
         const float thick = __expf(__uint_as_float(r[0])) * MIN_STEP * s;   // optical thickness of one minimal step
         density[gi] = fmaxf(density[gi] * decay, thick);
       }
     }
-    tc::tc_fence_before();
     __syncthreads();
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<64>(tmem);
 }
 
 }  // namespace ngp
@@ -803,18 +763,28 @@ int nslam_ngp_backward_tc(const nslam_ngp_model* m, const void* packed,
     configured = true;
   }
   cudaStream_t st = (cudaStream_t)stream;
+  float* dw_part = (float*)ngp_scratch(NGP_SCRATCH_DW, (size_t)num_sms * W_TOTAL * sizeof(float));
+  if (!dw_part) return (int)cudaErrorMemoryAllocation;
   backward_tc_kernel<<<num_sms, 128, smem, st>>>(coords, counters, (const __half2*)m->grid_half, lv,
                                                  (const unsigned char*)packed, (const unsigned char*)packed + PW_TOTAL,
-                                                 dout, m->mlp_grad, m->grid_grad, loss_scale, (const __half*)enc_in,
+                                                 dout, dw_part, m->grid_grad, loss_scale, (const __half*)enc_in,
                                                  (__half*)denc_scratch);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return (int)e;
+  dw_reduce_kernel<<<(W_TOTAL + 255) / 256, 256, 0, st>>>(dw_part, num_sms, m->mlp_grad);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return (int)e;
   if (denc_scratch) {
-    // one thread per (sample, level); the sample count lives on the device -> grid-stride over the capacity
+    // one thread per (sample, level); the sample count lives on the device -> grid-stride over the capacity.
+    // Gradients go to a fixed-point accumulator (order-independent sums) and are added to grid_grad afterwards.
+    const size_t n_vals = 2 * (size_t)m->n_grid;
+    long long* acc = (long long*)ngp_scratch(NGP_SCRATCH_GRID, n_vals * sizeof(long long));
+    if (!acc) return (int)cudaErrorMemoryAllocation;
     size_t want = (((size_t)max_samples + 31) / 32 * N_LEVELS * 32 + 255) / 256;
     const size_t cap = (size_t)num_sms * 32;
     grid_scatter_kernel<<<(unsigned)(want < cap ? want : cap), 256, 0, st>>>(coords, counters, (const __half*)denc_scratch, lv,
-                                                                            m->grid_grad, 1.f / loss_scale);
+                                                                            acc, 1.f / loss_scale);
+    fx_flush_kernel<<<(unsigned)(num_sms * 8), 256, 0, st>>>(acc, m->grid_grad, n_vals, 1.f / GRID_FX);
     e = cudaGetLastError();
   }
   return (int)e;

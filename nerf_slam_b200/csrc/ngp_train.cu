@@ -1,4 +1,4 @@
-// Path B — NeRF training step + rendering kernels (instant-NGP style), sm_100a.
+// Path B — NeRF training step + rendering kernels (instant-NGP style), sm_90a.
 //
 //   B3  one training step (what pyngp's Testbed.frame() does per call, fusion/nerf_fusion.py:299):
 //       sample rays over the training images -> occupancy-grid ray march -> hash-grid encode ->
@@ -150,8 +150,9 @@ __device__ __forceinline__ void make_ray(const Camera& c, float px, float py, fl
 // consecutive lattice points per iteration (one dependent bitfield load per 32 steps instead of one
 // per step): lane l rebuilds t_{base+l} with the same serial recurrence a single thread would run
 // (bit-identical t), the ballot of occupied points is kept in registers (lane c%32 holds chunk c),
-// the ray reserves its contiguous sample range with ONE atomicAdd, and the write pass replays the
-// kept masks without touching the bitfield again.  A sample is emitted for every lattice point that
+// the ray's contiguous sample range is either reserved with ONE atomicAdd (render) or given by the caller
+// (training: a count pass, an ordered scan, then this write pass, so that the sample layout is the same on every
+// run), and the write pass replays the kept masks without touching the bitfield again.  A sample is emitted for every lattice point that
 // lies in an occupied cell of its cascade, up to max_n samples / 4096 lattice points per ray.
 constexpr int MW_SLOTS = 4;                 // 4 x 32 chunks x 32 points
 
@@ -161,10 +162,12 @@ __device__ __forceinline__ float lattice_t(float tbase, int lane, float cone) {
   return t;
 }
 
-// returns the number of samples (uniform over the warp); writes them at coords/tdist[base...]
+// returns the number of samples (uniform over the warp); writes them at coords/tdist[base...].
+// base_in: -1 = reserve the range with an atomic on counters[0]; -2 = count only (nothing is written);
+// >= 0 = write at this offset
 __device__ int march_warp(const float* o, const float* d, const Scene& sc, const uint8_t* __restrict__ bits,
                           float jitter, int max_n, int max_samples, int* __restrict__ counters,
-                          float* __restrict__ coords, float* __restrict__ tdist, int& base_out) {
+                          float* __restrict__ coords, float* __restrict__ tdist, int& base_out, int base_in = -1) {
   const int lane = threadIdx.x & 31;
   const float id[3] = {1.f / d[0], 1.f / d[1], 1.f / d[2]};
   float tmin, tmax;
@@ -197,13 +200,15 @@ __device__ int march_warp(const float* o, const float* d, const Scene& sc, const
       tbase = __shfl_sync(0xffffffffu, t + dt, 31);
     }
   }
-  if (n == 0) return 0;
-  int base = 0;
-  if (lane == 0) {
-    base = atomicAdd(&counters[0], n);
-    if (base + n > max_samples) { atomicSub(&counters[0], n); base = -1; }
+  if (n == 0 || base_in == -2) return n;
+  int base = base_in;
+  if (base_in == -1) {
+    if (lane == 0) {
+      base = atomicAdd(&counters[0], n);
+      if (base + n > max_samples) { atomicSub(&counters[0], n); base = -1; }
+    }
+    base = __shfl_sync(0xffffffffu, base, 0);
   }
-  base = __shfl_sync(0xffffffffu, base, 0);
   if (base < 0) return 0;
   base_out = base;
   int off = 0, ci = 0;
@@ -231,15 +236,18 @@ __device__ int march_warp(const float* o, const float* d, const Scene& sc, const
 }
 
 // counters: [0] samples used, [1] rays kept, [2] rays tried.  One WARP per ray.
+// Two passes: count (R[13] = samples of ray i), then sample_scan_kernel, then write (at R[12], R[13] samples).
 __global__ void sample_rays_kernel(ImageStore st, Scene sc, const uint8_t* __restrict__ bits,
                                    int n_rays, uint32_t seed, int max_samples,
                                    float* __restrict__ rays, float* __restrict__ coords,
-                                   float* __restrict__ tdist, int* __restrict__ counters) {
+                                   float* __restrict__ tdist, int* __restrict__ counters, int count_pass) {
   const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (i >= n_rays) return;
   float* R = rays + (size_t)i * 16;
-  if (lane == 0) reinterpret_cast<int*>(R)[13] = 0;
-  if (st.n_active <= 0) return;
+  const int planned = count_pass ? 0 : reinterpret_cast<const int*>(R)[13];
+  __syncwarp();
+  if (count_pass && lane == 0) reinterpret_cast<int*>(R)[13] = 0;
+  if (st.n_active <= 0 || (!count_pass && planned == 0)) return;
   const int img = st.active[min((int)(rnd01(seed, i, 1) * st.n_active), st.n_active - 1)];
   const int px = min((int)(rnd01(seed, i, 2) * st.W), st.W - 1);
   const int py = min((int)(rnd01(seed, i, 3) * st.H), st.H - 1);
@@ -247,7 +255,12 @@ __global__ void sample_rays_kernel(ImageStore st, Scene sc, const uint8_t* __res
   make_ray(st.cams[img], px + 0.5f, py + 0.5f, o, d, inv_len);
   const float jit = rnd01(seed, i, 4);
   int base = 0;
-  const int n = march_warp(o, d, sc, bits, jit, MAX_STEPS, max_samples, counters, coords, tdist, base);
+  const int n = march_warp(o, d, sc, bits, jit, MAX_STEPS, max_samples, counters, coords, tdist, base,
+                           count_pass ? -2 : reinterpret_cast<const int*>(R)[12]);
+  if (count_pass) {
+    if (lane == 0) reinterpret_cast<int*>(R)[13] = n;
+    return;
+  }
   if (n == 0 || lane != 0) return;
   const size_t pix = ((size_t)img * st.H + py) * st.W + px;
   R[0] = o[0]; R[1] = o[1]; R[2] = o[2]; R[3] = d[0]; R[4] = d[1]; R[5] = d[2]; R[6] = inv_len;
@@ -259,7 +272,47 @@ __global__ void sample_rays_kernel(ImageStore st, Scene sc, const uint8_t* __res
   reinterpret_cast<int*>(R)[13] = n;
   reinterpret_cast<int*>(R)[14] = img;
   reinterpret_cast<int*>(R)[15] = py * st.W + px;
-  atomicAdd(&counters[1], 1);
+}
+
+// between the two passes of sample_rays_kernel: exclusive scan of the per-ray counts in ray order; rays are kept
+// while the running total fits max_samples (R[12] = offset, R[13] = count, 0 = dropped); counters[0] / [1] =
+// samples / rays kept.  One block.
+__global__ void __launch_bounds__(1024)
+sample_scan_kernel(float* __restrict__ rays, int n_rays, int max_samples, int* __restrict__ counters) {
+  __shared__ int wsum[32];
+  __shared__ int carry, kept, used;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  if (tid == 0) { carry = 0; kept = 0; used = 0; }
+  __syncthreads();
+  for (int c0 = 0; c0 < n_rays; c0 += 1024) {
+    const int i = c0 + tid;
+    int* R = reinterpret_cast<int*>(rays + (size_t)i * 16);
+    const int n = i < n_rays ? R[13] : 0;
+    int x = n;                                              // inclusive scan: warp, then across warps
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+    if (lane == 31) wsum[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+      int w = wsum[lane];
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += y; }
+      wsum[lane] = w;
+    }
+    __syncthreads();
+    const int incl = carry + x + (warp ? wsum[warp - 1] : 0);
+    const bool keep = n > 0 && incl <= max_samples;
+    if (i < n_rays) { R[12] = incl - n; R[13] = keep ? n : 0; }
+    if (keep) atomicMax(&used, incl);                       // kept rays form a prefix: the last one ends the range
+    const int nk = __syncthreads_count(keep);
+    if (tid == 1023) carry = incl;
+    if (tid == 0) kept += nk;
+    __syncthreads();
+  }
+  if (tid == 0) {
+    counters[0] = used;
+    counters[1] = kept;
+  }
 }
 
 // rays of one image tile (render): ray r <-> pixel (x0 + r % tw, y0 + r / tw).  One WARP per ray.
@@ -383,11 +436,13 @@ __device__ __forceinline__ float warp_scan_add(float v, int lane) {
   return v;
 }
 
+constexpr float LOSS_FX = 4294967296.f;            // 2^32: fixed-point scale of the batch-loss accumulator
+
 __global__ void loss_kernel(const float* __restrict__ rays, int n_rays, const float* __restrict__ coords,
                             const float* __restrict__ tdist, const float* __restrict__ rgbsigma,
                             const int* __restrict__ counters, float lambda_d, float3 bg, int mode,
                             float* __restrict__ dout, float* __restrict__ loss_acc,
-                            float* __restrict__ out_rgbd) {
+                            float* __restrict__ out_rgbd, long long* __restrict__ loss_fx = nullptr) {
   const int r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (r >= n_rays) return;
   const float* R = rays + (size_t)r * 16;
@@ -449,7 +504,10 @@ __global__ void loss_kernel(const float* __restrict__ rays, int n_rays, const fl
     loss += lambda_d * e * e / cov;
     ld = 2.f * lambda_d * e / cov * invR;
   }
-  if (lane == 0) atomicAdd(loss_acc, loss * invR);
+  if (lane == 0) {
+    if (loss_fx) fx_add(loss_fx, loss * invR, LOSS_FX);      // order-independent; added to loss_acc by fx_flush_kernel
+    else atomicAdd(loss_acc, loss * invR);
+  }
   // ---- backward sweep
   float T2 = 1.f, r2 = 0.f, g2 = 0.f, b2 = 0.f, d2 = 0.f;       // carries: values after the previous chunk
   for (int c0 = 0; c0 < n; c0 += 32) {
@@ -651,7 +709,7 @@ density_sample_kernel(const __half2* __restrict__ grid, LevelInfo lv, const floa
   if (i >= total) return;
   const int mip = i / n_per_cascade, j = i % n_per_cascade;
   const int NC = GRID * GRID * GRID;
-  const uint32_t cell = (n_per_cascade >= NC) ? (uint32_t)j : (pcg(pcg(seed) ^ (uint32_t)i) % NC);
+  const uint32_t cell = (n_per_cascade >= NC) ? (uint32_t)j : density_cell(seed, mip, j);
   const size_t gi = (size_t)mip * NC + cell;
   if (density[gi] < 0.f) return;   // never visible from a training camera
   const int ix = cell % GRID, iy = (cell / GRID) % GRID, iz = cell / (GRID * GRID);
@@ -704,15 +762,32 @@ __global__ void density_mark_kernel(const Camera* __restrict__ cams, const int* 
   }
 }
 
-// mean of the non-negative densities -> stats[0] = sum, stats[1] = count
-__global__ void density_mean_kernel(const float* __restrict__ density, size_t n, float* __restrict__ stats) {
+// mean of the non-negative densities -> stats[0] = sum, stats[1] = count.  Fixed summation order (no atomics):
+// each block writes its partial, density_mean_final_kernel adds the partials in block order.
+constexpr int DM_BLOCKS = 592;
+__device__ float g_density_partials[2 * DM_BLOCKS];
+__global__ void __launch_bounds__(256) density_mean_kernel(const float* __restrict__ density, size_t n) {
+  __shared__ float ws[2][8];
   float s = 0.f, c = 0.f;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const float d = density[i];
     if (d >= 0.f) { s += d; c += 1.f; }
   }
   for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); c += __shfl_xor_sync(0xffffffffu, c, o); }
-  if ((threadIdx.x & 31) == 0) { atomicAdd(&stats[0], s); atomicAdd(&stats[1], c); }
+  if ((threadIdx.x & 31) == 0) { ws[0][threadIdx.x >> 5] = s; ws[1][threadIdx.x >> 5] = c; }
+  __syncthreads();
+  if (threadIdx.x < 2) {
+    float v = 0.f;
+    for (int w = 0; w < 8; w++) v += ws[threadIdx.x][w];
+    g_density_partials[2 * blockIdx.x + threadIdx.x] = v;
+  }
+}
+__global__ void density_mean_final_kernel(float* __restrict__ stats) {
+  if (threadIdx.x < 2) {
+    float v = 0.f;
+    for (int b = 0; b < DM_BLOCKS; b++) v += g_density_partials[2 * b + threadIdx.x];
+    stats[threadIdx.x] = v;
+  }
 }
 __global__ void density_bits_kernel(const float* __restrict__ density, size_t nbytes,
                                     const float* __restrict__ stats, float min_thick,
@@ -842,6 +917,16 @@ extern "C" {
 
 /* one training step WITHOUT the optimiser: sample rays, march, forward, loss, backward.
  * Gradients accumulate into model->*_grad (must be zero on entry; nslam_ngp_adam zeroes them). */
+static void sample_rays(const nslam_ngp_model* m, const nslam_ngp_images* im, const nslam_ngp_batch* b, int n_rays,
+                        unsigned seed, cudaStream_t st) {
+  using namespace ngp;
+  for (int pass = 1; pass >= 0; pass--) {
+    sample_rays_kernel<<<(n_rays + 3) / 4, 128, 0, st>>>(make_store(im), make_scene(m), m->bits, n_rays, seed,
+                                                           b->max_samples, b->rays, b->coords, b->tdist, b->counters, pass);
+    if (pass) sample_scan_kernel<<<1, 1024, 0, st>>>(b->rays, n_rays, b->max_samples, b->counters);
+  }
+}
+
 int nslam_ngp_train_step(const nslam_ngp_model* m, const nslam_ngp_images* im, const nslam_ngp_batch* b,
                          int n_rays, unsigned seed, float lambda_depth, float bg_r, float bg_g,
                          float bg_b, int num_sms, void* stream) {
@@ -854,15 +939,17 @@ int nslam_ngp_train_step(const nslam_ngp_model* m, const nslam_ngp_images* im, c
   cudaMemsetAsync(b->loss, 0, sizeof(float), st);
   const LevelInfo lv = make_lv(m);
   const Scene sc = make_scene(m);
-  sample_rays_kernel<<<(n_rays + 3) / 4, 128, 0, st>>>(make_store(im), sc, m->bits, n_rays, seed,
-                                                         b->max_samples, b->rays, b->coords, b->tdist, b->counters);
+  sample_rays(m, im, b, n_rays, seed, st);
   NGP_CHECK_LAUNCH();
   forward_kernel<<<(b->max_samples + TILE - 1) / TILE, TILE, FWD_SMEM, st>>>(
       b->coords, b->counters, -1, (const __half2*)m->grid_half, lv, m->mlp, b->rgbsigma);
   NGP_CHECK_LAUNCH();
+  long long* loss_fx = (long long*)ngp_scratch(NGP_SCRATCH_LOSS, sizeof(long long));
+  if (!loss_fx) return (int)cudaErrorMemoryAllocation;
   loss_kernel<<<(n_rays + 3) / 4, 128, 0, st>>>(b->rays, n_rays, b->coords, b->tdist, b->rgbsigma,
                                                      b->counters, lambda_depth, make_float3(bg_r, bg_g, bg_b),
-                                                     0, b->dout, b->loss, nullptr);
+                                                     0, b->dout, b->loss, nullptr, loss_fx);
+  fx_flush_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(loss_fx, b->loss, 1, 1.f / LOSS_FX);
   NGP_CHECK_LAUNCH();
   backward_kernel<<<2 * num_sms, TILE, BWD_SMEM, st>>>(b->coords, b->counters, (const __half2*)m->grid_half,
                                                        lv, m->mlp, b->dout, m->mlp_grad, m->grid_grad);
@@ -879,8 +966,7 @@ int nslam_ngp_sample_phase(const nslam_ngp_model* m, const nslam_ngp_images* im,
   if (n_rays > b->max_rays) return (int)cudaErrorInvalidValue;
   cudaMemsetAsync(b->counters, 0, 4 * sizeof(int), st);
   cudaMemsetAsync(b->loss, 0, sizeof(float), st);
-  sample_rays_kernel<<<(n_rays + 3) / 4, 128, 0, st>>>(make_store(im), make_scene(m), m->bits, n_rays, seed,
-                                                         b->max_samples, b->rays, b->coords, b->tdist, b->counters);
+  sample_rays(m, im, b, n_rays, seed, st);
   NGP_CHECK_LAUNCH();
   return 0;
 }
@@ -888,9 +974,12 @@ int nslam_ngp_sample_phase(const nslam_ngp_model* m, const nslam_ngp_images* im,
 int nslam_ngp_loss_phase(const nslam_ngp_batch* b, int n_rays, float lambda_depth, float bg_r, float bg_g,
                          float bg_b, void* stream) {
   using namespace ngp;
+  long long* loss_fx = (long long*)ngp_scratch(NGP_SCRATCH_LOSS, sizeof(long long));
+  if (!loss_fx) return (int)cudaErrorMemoryAllocation;
   loss_kernel<<<(n_rays + 3) / 4, 128, 0, (cudaStream_t)stream>>>(b->rays, n_rays, b->coords, b->tdist, b->rgbsigma,
                                                                        b->counters, lambda_depth,
-                                                                       make_float3(bg_r, bg_g, bg_b), 0, b->dout, b->loss, nullptr);
+                                                                       make_float3(bg_r, bg_g, bg_b), 0, b->dout, b->loss, nullptr, loss_fx);
+  fx_flush_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(loss_fx, b->loss, 1, 1.f / LOSS_FX);
   NGP_CHECK_LAUNCH();
   return 0;
 }
@@ -938,8 +1027,11 @@ int nslam_ngp_loss_backward(const nslam_ngp_model* m, const nslam_ngp_batch* b, 
   forward_kernel<<<(n_samples + TILE - 1) / TILE, TILE, FWD_SMEM, st>>>(b->coords, b->counters, -1,
                                                                        (const __half2*)m->grid_half, lv, m->mlp, b->rgbsigma);
   NGP_CHECK_LAUNCH();
+  long long* loss_fx = (long long*)ngp_scratch(NGP_SCRATCH_LOSS, sizeof(long long));
+  if (!loss_fx) return (int)cudaErrorMemoryAllocation;
   loss_kernel<<<(n_rays + 3) / 4, 128, 0, st>>>(b->rays, n_rays, b->coords, b->tdist, b->rgbsigma, b->counters,
-                                                     lambda_depth, make_float3(bg_r, bg_g, bg_b), 0, b->dout, b->loss, nullptr);
+                                                     lambda_depth, make_float3(bg_r, bg_g, bg_b), 0, b->dout, b->loss, nullptr, loss_fx);
+  fx_flush_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(loss_fx, b->loss, 1, 1.f / LOSS_FX);
   NGP_CHECK_LAUNCH();
   backward_kernel<<<2 * num_sms, TILE, BWD_SMEM, st>>>(b->coords, b->counters, (const __half2*)m->grid_half, lv,
                                                        m->mlp, b->dout, m->mlp_grad, m->grid_grad);
@@ -969,8 +1061,8 @@ int nslam_ngp_update_density_grid(const nslam_ngp_model* m, const nslam_ngp_imag
                                                                        make_scene(m), n_per_cascade, seed, decay, m->density);
     NGP_CHECK_LAUNCH();
   }
-  cudaMemsetAsync(m->stats, 0, 2 * sizeof(float), st);
-  density_mean_kernel<<<592, 256, 0, st>>>(m->density, total, m->stats);
+  density_mean_kernel<<<DM_BLOCKS, 256, 0, st>>>(m->density, total);
+  density_mean_final_kernel<<<1, 32, 0, st>>>(m->stats);
   NGP_CHECK_LAUNCH();
   density_bits_kernel<<<(unsigned)((total / 8 + 255) / 256), 256, 0, st>>>(m->density, total / 8, m->stats,
                                                                           min_thickness, m->bits);

@@ -1,7 +1,7 @@
-// Blackwell (sm_100a) primitives used by the tensor-core kernels: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld) and UMMA descriptors.
-// Raw inline PTX — no CUTLASS dependency.  Bit layouts follow the PTX ISA "tcgen05" chapter
-// (shared-memory matrix descriptor, instruction descriptor for .kind::f16).
+// Hopper (sm_90a) primitives used by the tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor),
+// warpgroup MMA (wgmma.mma_async) and its shared-memory matrix descriptors.
+// Raw inline PTX — no CUTLASS dependency.  Bit layouts follow the PTX ISA "warpgroup-level matrix
+// multiply-accumulate" chapter (matrix descriptor, register fragments of the f32 accumulator).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -108,231 +108,112 @@ __device__ __forceinline__ void bulk_copy_g2s_lead(void* dst, const void* src, u
       : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---------------------------------------------------------------- wgmma
+// One warpgroup (4 consecutive warps, the first a multiple of 4) issues each wgmma collectively:
+//   D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, fp16 inputs from shared memory (both K-major), fp32 accumulator in
+//   registers.  Fragment of thread t of the warpgroup (warp w = t / 32, lane l):
+//     d[4 * j + 2 * i + c] = D[16 * w + l / 4 + 8 * i][8 * j + 2 * (l % 4) + c]      (i, c in {0, 1}, j < N / 8)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across wgmma issue and wait
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], fp16/bf16 inputs, fp32 accumulate
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                         uint32_t idesc, uint32_t accumulate) {
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate);
+template <>
+__device__ __forceinline__ void wgmma_f16<16>(float (&d)[8], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// arrive on an mbarrier once all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
+template <>
+__device__ __forceinline__ void wgmma_f16<32>(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-          smem_u32(bar))
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// WARP-UNIFORM issue (all 32 lanes execute the surrounding loop, the instruction itself is predicated on `lead`, e.g.
-// lead = elect_one()).  A tcgen05.mma issued from inside `if (lane == 0)` makes the compiler treat descriptors, loop
-// counters and barrier addresses as divergent values: every MMA is then preceded by an ELECT / R2UR.BROADCAST /
-// BRA.U.ANY loop that moves them into uniform registers — ~25 dependent instructions, ~90 cycles per MMA, more than the
-// 64 cycles an M128 x N128 x K16 MMA takes (profiles/r02_conv_analysis.md).  In uniform control flow the operands stay
-// in uniform registers and an MMA costs a handful of instructions.
-__device__ __forceinline__ void umma_f16_lead(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate, uint32_t lead) {
+template <>
+__device__ __forceinline__ void wgmma_f16<40>(float (&d)[20], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "setp.ne.b32 q, %5, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(lead)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %22, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n40k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19}, %20, %21, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit_lead(uint64_t* bar, uint32_t lead) {
+template <>
+__device__ __forceinline__ void wgmma_f16<64>(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred q;\n\t"
-      "setp.ne.b32 q, %1, 0;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(smem_u32(bar)),
-      "r"(lead)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// 32 lanes x 32 columns of 32-bit: thread i of the warp gets lane (base_lane+i), columns c..c+31
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t* r) {
+template <>
+__device__ __forceinline__ void wgmma_f16<128>(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// 32 lanes x 8 columns
-__device__ __forceinline__ void tmem_ld_32x8(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-      : "r"(taddr)
-      : "memory");
+
+// Fragment columns [8 * j_lo, 8 * j_hi) of an m64nN accumulator -> fp32 shared tile rows row0 + [0, 64), columns from
+// col0: the row-per-thread epilogues read their rows back from there.  `wtid` = thread index in the warpgroup.
+template <int N>
+__device__ __forceinline__ void acc_to_smem(float* tile, int ld, int row0, int col0, const float (&d)[N / 2], int wtid,
+                                            int j_lo = 0, int j_hi = N / 8) {
+  const int w = wtid >> 5, l = wtid & 31;
+  float* base = tile + (size_t)(row0 + 16 * w + (l >> 2)) * ld + col0 + 2 * (l & 3);
+#pragma unroll
+  for (int j = 0; j < N / 8; j++) {
+    if (j < j_lo || j >= j_hi) continue;
+    float* p = base + 8 * (j - j_lo);
+    *reinterpret_cast<float2*>(p) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(p + 8 * ld) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
 }
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// NC consecutive fp32 values of one row of a shared tile, as raw bits (the accumulator row of one thread)
+template <int NC>
+__device__ __forceinline__ void smem_row_ld(const float* tile, int ld, int row, int col, uint32_t* r) {
+  const float4* p = reinterpret_cast<const float4*>(tile + (size_t)row * ld + col);
+#pragma unroll
+  for (int i = 0; i < NC / 4; i++) {
+    const float4 v = p[i];
+    r[4 * i] = __float_as_uint(v.x); r[4 * i + 1] = __float_as_uint(v.y);
+    r[4 * i + 2] = __float_as_uint(v.z); r[4 * i + 3] = __float_as_uint(v.w);
+  }
+}
+// named barrier over `count` threads (e.g. one warpgroup)
+__device__ __forceinline__ void named_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 // Shared-memory matrix descriptor, K-major operand, 128-byte swizzle:
 //   rows of 128 B (64 fp16), 8-row groups 1024 B apart (SBO), base 1024-B aligned.
 //   bits [0,14) addr>>4 | [16,30) LBO>>4 (=1, unused for swizzled K-major) | [32,46) SBO>>4 (=64)
-//   | [46,48) version = 1 (Blackwell) | [61,64) layout type = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+//   | [62,64) layout type = 1 (SWIZZLE_128B)
+// Advancing K by 16 elements inside the swizzle atom = +32 B = +2 in the address field.
+__device__ __forceinline__ uint64_t desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)64 << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
-}
-// the same with an explicit stride between 8-row groups (SBO, bytes, multiple of 16): e.g. the rows of a pixel tile that
-// sits inside a wider halo box.  The start address may be any 128-byte row of a 1024-byte-aligned swizzled buffer.
-__device__ __forceinline__ uint64_t umma_desc_sw128_sbo(uint32_t smem_addr, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(sbo_bytes >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-// Instruction descriptor for kind::f16: D=f32, A/B = f16 (0) or bf16 (1), both K-major.
-//   [4,6) c_format=1 (F32) | [7,10) a_format | [10,13) b_format | [15] a_major=0 | [16] b_major=0
-//   | [17,23) N>>3 | [24,29) M>>4
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N, int ab_format) {
-  return (1u << 4) | ((uint32_t)ab_format << 7) | ((uint32_t)ab_format << 10) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// ---------------------------------------------------------------- CTA pairs (cta_group::2)
-// Two CTAs of a cluster (ranks 2k, 2k+1: the two SMs of a TPC) execute ONE tcgen05.mma of M = 256: each CTA
-// supplies its own 128 rows of A and HALF of the B tile (N/2 rows) from the same shared-memory offsets, and
-// receives its own 128 x N accumulator rows in its own TMEM.  The even ("leader") CTA issues the MMAs; loads of
-// both CTAs complete on the LEADER's mbarriers, commits are multicast to the barriers of both CTAs.
-// Shared-window addresses of the odd CTA differ from the even CTA's in bit 24 only.
-constexpr uint32_t PEER_BIT_MASK = 0xFEFFFFFFu;
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the barrier at the same offset in the leader (even) CTA of the pair — from either CTA
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & PEER_BIT_MASK)
-               : "memory");
-}
-// TMA loads into the executing CTA's shared memory that complete on the LEADER CTA's mbarrier
-__device__ __forceinline__ void tma_load_4d_pair(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                                 int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, "
-      "{%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(m), "r"(smem_u32(bar) & PEER_BIT_MASK), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, "
-      "{%3, %4}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(m), "r"(smem_u32(bar) & PEER_BIT_MASK), "r"(c0), "r"(c1)
-      : "memory");
-}
-// warp-uniform variants (whole warp in the loop, `lead` lane issues)
-__device__ __forceinline__ void tma_load_4d_pair_lead(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                                      int c3, uint32_t lead) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %7, 0;\n\t"
-      "@q cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, "
-      "{%3, %4, %5, %6}], [%2];\n\t}" ::"r"(smem_u32(dst)),
-      "l"(m), "r"(smem_u32(bar) & PEER_BIT_MASK), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(lead)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_pair_lead(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, uint32_t lead) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %5, 0;\n\t"
-      "@q cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, "
-      "{%3, %4}], [%2];\n\t}" ::"r"(smem_u32(dst)),
-      "l"(m), "r"(smem_u32(bar) & PEER_BIT_MASK), "r"(c0), "r"(c1), "r"(lead)
-      : "memory");
-}
-// TMEM: the same warp of BOTH CTAs allocates / frees (one collective operation of the pair)
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* dst_smem) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[256 rows: 128 per CTA] * B[N: N/2 per CTA]; issued by one thread of the leader CTA
-__device__ __forceinline__ void umma_f16_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on the barrier at this offset in BOTH CTAs once all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"((uint16_t)3)
-      : "memory");
-}
-
-// warp-uniform variants (see umma_f16_lead)
-__device__ __forceinline__ void umma_f16_pair_lead(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                                   uint32_t accumulate, uint32_t lead) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "setp.ne.b32 q, %5, 0;\n\t"
-      "@q tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(lead)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_pair_lead(uint64_t* bar, uint32_t lead) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\t"
-      "setp.ne.b32 q, %2, 0;\n\t"
-      "@q tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t}" ::"r"(
-          smem_u32(bar)),
-      "h"((uint16_t)3), "r"(lead)
-      : "memory");
 }
 
 __device__ __forceinline__ bool elect_one() {

@@ -12,7 +12,7 @@
 //     wr = weight_reading[v,u];  wp = w + wr                                                            (:274-277)
 //     tsdf = (w tsdf + wr sdf) / wp;  color = (w color + wr rgb) / wp;  w = min(wp, max_weight)         (:280-294)
 //
-// B200 design: 180 GB of HBM make the hashing unnecessary for the reference's own extent ("a 6 m room with a dense
+// Design: 80 GB of HBM make the hashing unnecessary for the reference's own extent ("a 6 m room with a dense
 // 512^3 grid", :66) — the volume is a DENSE grid (tsdf, weight fp32 + colour 3 x fp32 = 20 B/voxel, 2.7 GB at 512^3),
 // one thread per voxel, one launch per keyframe; depth = 1 / inverse depth, weight = 1 / sqrt(depth variance) and the
 // depth mask are evaluated on the fly from the packet's tensors (the reference materialises three images per frame).

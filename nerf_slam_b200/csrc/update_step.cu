@@ -41,8 +41,9 @@ extern "C" int nslam_update_op_step(const nslam_update_ctx* c, void* stream) {
   int r;
   auto conv = [&](const void* const* srcs, const int* ch, int ns, int B, int k, int N, int wi, int mode, int act,
                   const float* gctx, const void* net, const void* zbuf, float* gsum, void* out0, int oc, void* out1) {
+    // mode 3 (glo): its per-tile partials live behind gsum[E][128] in the same workspace slice
     return nslam_conv_igemm(srcs, ch, ns, B, H, W, k, k, k / 2, N, c->wp[wi], c->bias[wi], mode, act, gctx, net, zbuf, gsum,
-                            out0, oc, out1, S, stream);
+                            out0, oc, out1, mode == 3 ? gsum + (size_t)B * 128 : nullptr, S, stream);
   };
   // correlation / motion encoders
   { const void* s[1] = {c->corr}; int ch[1] = {c->corr_channels};

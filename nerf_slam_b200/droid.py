@@ -1,4 +1,4 @@
-"""DROID-style plugin surface of the reference on top of the sm_100a kernels (SURVEY.md §8 row A19 "API twins",
+"""DROID-style plugin surface of the reference on top of the sm_90a kernels (SURVEY.md §8 row A19 "API twins",
 §8b "Python class surface to keep"):
 
   DroidNet                      .feature_net/.fnet  .context_net/.cnet  .update_net/.update   (networks/droid_net.py:153-158)
@@ -12,11 +12,11 @@
 The reference ships these classes without the `video` they need and with one hole (`gru_contexts_input` is
 never filled, networks/factor_graph.py:128-131 vs :219-220); both are closed here.
 
-Layout decisions (B200-first, not the reference's):
+Layout decisions (GPU-first, not the reference's):
   * edge lists are CONTROL data and live on the host (`ii`, `jj`, `age`, ... are CPU int64 tensors sharing
     memory with numpy arrays); device copies are made once per edge-set change.  The reference keeps them
     on the GPU and pays a device->host sync for every `.item()` in its Python loops.
-  * per-edge state is channels-last fp16 (`[E,ht,wd,128]`, the tcgen05 operand layout); the reference-shaped
+  * per-edge state is channels-last fp16 (`[E,ht,wd,128]`, the wgmma operand layout); the reference-shaped
     `[1,E,128,ht,wd]` tensors are exposed as views.
   * correlation volumes sit in a slot arena (`CorrPool`): adding/removing edges never copies volumes.
 Every kernel call goes through `droid_backends` / `conv` (the C-ABI library); nothing here computes on the CPU.
@@ -107,7 +107,7 @@ class EncoderNetTC:
 
 
 class UpdateNetTC:
-    """UpdateModule.forward's convention (networks/droid_net.py:118-150) on the fused tcgen05 update operator:
+    """UpdateModule.forward's convention (networks/droid_net.py:118-150) on the fused tensor-core update operator:
     net, inp [1,E,128,ht,wd]; corr [1,E,196,ht,wd]; flow [1,E,4,ht,wd] | None; ii (GraphAgg) | None
       -> net [1,E,128,ht,wd], delta [1,E,ht,wd,2], weight [1,E,ht,wd,2] (, eta [1,K,ht,wd], upmask [1,K,576,ht,wd]).
     `fused` is the channels-last operator itself; `FactorGraph` calls it directly (no layout round trip)."""

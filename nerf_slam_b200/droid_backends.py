@@ -2,7 +2,7 @@
 
 Same 12 function names, argument order, tensor layouts, in-place semantics and error behaviour
 as the pybind module defined at reference src/droid.cpp:347-363 — but every function forwards to
-a hand-written sm_100a kernel through the C ABI of libnslam_sm100a.so (include/nslam.h).
+a hand-written sm_90a kernel through the C ABI of libnslam_sm90a.so (include/nslam.h).
 `import nerf_slam_b200.droid_backends as droid_backends` (or put `nerf_slam_b200/shim` on
 sys.path) and the reference's networks/modules/corr.py + visual_frontend.py run unchanged.
 
@@ -49,7 +49,7 @@ def _chk(*ts):
         if not t.is_contiguous():
             raise RuntimeError("tensor must be contiguous")  # CHECK_CONTIGUOUS, src/droid.cpp:129
         if not t.is_cuda:
-            raise RuntimeError("droid_backends (sm_100a) needs CUDA tensors; there is no CPU path")
+            raise RuntimeError("droid_backends (sm_90a) needs CUDA tensors; there is no CPU path")
 
 
 def _i64(t):

@@ -1,5 +1,5 @@
 """RaftVisualFrontend — the live SLAM front-end of the reference
-(slam/visual_frontends/visual_frontend.py:62-1391) re-hosted on the sm_100a kernels.
+(slam/visual_frontends/visual_frontend.py:62-1391) re-hosted on the sm_90a kernels.
 
 Same public surface: RaftVisualFrontend(world_T_body_t0, body_T_cam0, args, device)
   .forward(batch) -> (x0, factors, viz_out)      .update(...)      .ba(...)      .stop_condition()
@@ -8,10 +8,10 @@ Same algorithm and constants (SURVEY.md §5 "Config", §9): warm-up 8 keyframes,
 max 48 factors, max age 25, 4+2 update iterations, keyframe threshold 4.0, BA window
 kf0 = max(0, min(ii)), 1e-4-sigma prior on frame 0, inactive edges >= kf0-3 prepended.
 
-What is different (B200 design, not a translation):
+What is different (GPU-first design, not a translation):
   * state lives in pre-allocated device arenas; correlation pyramids in a slot pool (CorrPool)
     so edges are added/removed without re-copying volumes (reference: torch.cat per add);
-  * features are stored channels-last fp16 — the layout the tcgen05 kernels consume;
+  * features are stored channels-last fp16 — the layout the tensor-core kernels consume;
   * the whole BA iteration (linearise -> Schur -> dense fp64 Cholesky -> SE3 retract -> depth
     update -> covariances) runs on the GPU stream: no Eigen, no gtsam, no per-block
     .cpu().numpy() HessianFactor loop, no host synchronisation inside update();
@@ -193,7 +193,7 @@ class RaftVisualFrontend:
             self.weights_source = wpath
         for m in (self.feature_net, self.context_net, self.update_net):
             m.to(device=device, dtype=torch.float16)
-        # encoders and update operator: hand-written tcgen05 implicit-GEMM convolutions.  There is no library / CPU
+        # encoders and update operator: hand-written wgmma implicit-GEMM convolutions.  There is no library / CPU
         # alternative in the product (the cuDNN formulation of the same networks lives with the reference arm,
         # oracle/ref_cuda_frontend.py, and in the parity tests).
         from .conv import EncoderTC, UpdateOperatorTC
@@ -279,7 +279,7 @@ class RaftVisualFrontend:
         self.prior_pose = torch.tensor(self.world_T_cam0_t0, **f)   # prior mean (visual_frontend.py:1235)
         cams = 2 if self.stereo else 1
         self.cameras = cams
-        # features channels-last fp16 (tcgen05 operand layout); contexts channels-first views of NHWC storage
+        # features channels-last fp16 (wgmma operand layout); contexts channels-first views of NHWC storage
         self.features_imgs = torch.zeros(B, cams, ht, wd, 128, dtype=torch.float16, device=dev)
         self.contexts_imgs = torch.zeros(B, cams, ht, wd, 128, dtype=torch.float16, device=dev)       # NHWC
         self.cst_contexts_imgs = torch.zeros(B, cams, ht, wd, 128, dtype=torch.float16, device=dev)   # NHWC

@@ -1,4 +1,4 @@
-"""NerfFusion — the reference's fusion/nerf_fusion.py:29-485 on the sm_100a NeRF kernels.
+"""NerfFusion — the reference's fusion/nerf_fusion.py:29-485 on the sm_90a NeRF kernels.
 
 Same surface: NerfFusion(name, args, device) .fuse(data_packets) .stop_condition()
               .process_slam / .process_data / .send_data / .fit_volume / .fit_volume_once / .eval_gt_traj

@@ -1,4 +1,4 @@
-"""`pyngp`-shaped façade over the sm_100a NeRF kernels (Path B).
+"""`pyngp`-shaped façade over the sm_90a NeRF kernels (Path B).
 
 Exposes exactly the surface that the reference's fusion/nerf_fusion.py uses of the instant-ngp
 fork's python module (SURVEY.md §8b "pyngp surface used"):
@@ -180,7 +180,8 @@ class Testbed:
         self._measured = None
         self.grad_hook = None        # e.g. dist.allreduce_grads for data-parallel training
         self._ctr_event = None; self._ctr_host = None; self._loss_host = None; self._ctr_rays = 0
-        # "tcgen05": MLP forward/backward on tensor cores (csrc/ngp_tc.cu); "simt": fp32 CUDA-core kernels
+        # "tcgen05" (the historical name of the tensor-core path): MLP forward/backward on tensor cores (wgmma,
+        # csrc/ngp_tc.cu); "simt": fp32 CUDA-core kernels
         self.mlp_backend = "tcgen05"
         self.loss_scale = 1024.0
 
@@ -253,7 +254,7 @@ class Testbed:
         self.pack_weights()
 
     def pack_weights(self):
-        """fp16 UMMA-ready images of the current fp32 MLP weights (after init / every optimiser step)"""
+        """fp16 wgmma-ready images of the current fp32 MLP weights (after init / every optimiser step)"""
         _lib.check(_lib.load().nslam_ngp_pack_mlp(_lib.ptr(self.mlp), _lib.ptr(self.packed), _lib.stream_ptr()), "ngp_pack_mlp")
 
     def _ensure_store(self, H, W):
@@ -349,7 +350,8 @@ class Testbed:
                                               lv["size"].ctypes.data, lv["offset"].ctypes.data, lv["dense"].ctypes.data,
                                               float(self.aabb_scale), _lib.ptr(self._bufs["rays"]), int(self.rays_per_batch),
                                               _lib.ptr(self._bufs["coords"]), _lib.ptr(self._bufs["tdist"]), _lib.ptr(self._bufs["denc"]),
-                                              float(self.loss_scale), _lib.ptr(self.cam_grad), _lib.stream_ptr()), "ngp_cam_grad")
+                                              float(self.loss_scale), _lib.ptr(self.cam_grad), int(self.cam_grad.shape[0]),
+                                              _lib.stream_ptr()), "ngp_cam_grad")
         if self.grad_hook is not None:
             self.grad_hook(self)
         if refine:

@@ -1,5 +1,5 @@
 """TsdfFusion — the reference's fusion/tsdf_fusion.py (`--fusion=tsdf` / `--fusion=sigma`, SURVEY.md §8 f3) on a dense
-sm_100a voxel grid.
+sm_90a voxel grid.
 
 Same surface: TsdfFusion(name, args, device)  .fuse(data_packets)  .stop_condition()
               .handle_slam_packet / .update_history / .get_history_packet / .get_depth_masks / .build_volume /
@@ -9,7 +9,7 @@ name "tsdf": uniform weights; "sigma": weights 1 / sqrt(depth variance) from the
 
 Differences by design: Open3D's hashed VoxelBlockGrid driven from Python (~40 tensor ops and four device
 synchronisations per keyframe, :185-302) becomes one kernel launch per keyframe on a DENSE grid (csrc/tsdf.cu) —
-the reference's own extent "6 m / 512 voxels" is 2.7 GB at 20 B per voxel on a 180 GB part; poses, depths, weights and
+the reference's own extent "6 m / 512 voxels" is 2.7 GB at 20 B per voxel on an 80 GB part; poses, depths, weights and
 masks are consumed where the SLAM packet holds them (device tensors; the reference converts each frame to three Open3D
 images and copies the poses to the host)."""
 import numpy as np

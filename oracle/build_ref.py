@@ -1,6 +1,6 @@
 """ORACLE build recipe (test infrastructure only).
 
-Compiles the reference's OWN CUDA kernels for sm_100a, from the sources where they lie under
+Compiles the reference's OWN CUDA kernels for sm_90a, from the sources where they lie under
 /root/reference, into oracle/_ref/*.so (git-ignored, but shipped to the GPU box by gpurun):
 
   nslam_ref_corr.so   src/correlation_kernels.cu + src/altcorr_kernel.cu, with the 3-token
@@ -13,7 +13,7 @@ Compiles the reference's OWN CUDA kernels for sm_100a, from the sources where th
 
 Patched intermediates go to a temp dir outside the repo; no reference source is copied into the
 tree.  Used to (a) pin the CPU oracle and the CUDA product path against the reference kernels on
-a B200 (tests/test_gpu_vs_reference.py), (b) generate tests/golden/*.npz, (c) time the
+the GPU (tests/test_gpu_vs_reference.py), (b) generate tests/golden/*.npz, (c) time the
 reference's CUDA build next to ours (bench.py --impl reference-cuda).
 """
 import os
@@ -33,7 +33,7 @@ def _build(name, sources, tmp):
     bdir = os.path.join(tmp, name)
     os.makedirs(bdir, exist_ok=True)
     cpp_extension.load(name=name, sources=sources, build_directory=bdir, verbose=False,
-                       extra_cuda_cflags=["-O3", "-gencode", "arch=compute_100a,code=sm_100a"],
+                       extra_cuda_cflags=["-O3", "-gencode", "arch=compute_90a,code=sm_90a"],
                        is_python_module=False)
     os.makedirs(OUT, exist_ok=True)
     shutil.copy(os.path.join(bdir, name + ".so"), os.path.join(OUT, name + ".so"))

@@ -5,7 +5,7 @@ CPU restatements of the correlation operators of the reference:
   A3  corr_index_forward_kernel                    src/correlation_kernels.cu:19-70
   A4  altcorr_forward_kernel + AltCorrBlock        src/altcorr_kernel.cu:27-149, networks/modules/corr.py:92-126
 Pinned by tests/golden/ (reference python modules imported on CPU, reference CUDA kernels run on
-a B200 from oracle/_ref) — see tests/golden/README.md.
+the GPU from oracle/_ref) — see tests/golden/README.md.
 """
 import numpy as np
 

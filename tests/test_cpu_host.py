@@ -11,7 +11,7 @@ from oracle import se3 as ose3
 
 def test_pack_weights_layout():
     """packed image = [tap][source][64-channel block] blocks of [N_pad][64] fp16, 16-byte chunk j of row n stored at
-    chunk position j ^ (n & 7)  (the 128-byte swizzle the UMMA shared-memory descriptor expects)"""
+    chunk position j ^ (n & 7)  (the 128-byte swizzle the wgmma shared-memory descriptor expects)"""
     from nerf_slam_b200.conv import pack_weights
     g = torch.Generator().manual_seed(0)
     for (N, srcs, k, npad) in ((16, [128], 3, None), (128, [128, 128, 128, 64], 3, None), (32, [152], 1, None),
@@ -121,199 +121,6 @@ def test_halo_tile_schedule_reproduces_the_convolution():
     assert float((got - ref).abs().max()) < 2e-3
 
 
-# ---------------------------------------------------------------------------------------------------------------
-# csrc/conv_igemm2.cu (CTA pairs, tcgen05 cta_group::2): discrete-event emulation of the synchronisation protocol.
-# Every actor below follows the kernel's loops and index arithmetic line for line (stage = counter % depth,
-# parity = (counter / depth) & 1, "empty" waits use parity ^ 1); loads and MMAs complete asynchronously after random
-# delays; the scheduler interleaves the actors at random.  Checked: no deadlock, every MMA sees the tile / weight
-# half it expects in BOTH CTAs, no stage is overwritten while an issued MMA may still read it, no accumulator stage
-# is overwritten before both epilogues have drained it, every epilogue reads the accumulator of its own pair.
-class _MBar:
-    def __init__(self, count):
-        self.count, self.pending, self.tx, self.phase = count, count, 0, 0
-
-    def _maybe_flip(self):
-        if self.pending == 0 and self.tx == 0:
-            self.phase ^= 1
-            self.pending = self.count
-
-    def arrive(self, tx=0):
-        self.tx += tx
-        self.pending -= 1
-        assert self.pending >= 0, "more arrivals than the barrier was initialised for"
-        self._maybe_flip()
-
-    def complete_tx(self, nbytes):
-        self.tx -= nbytes
-        self._maybe_flip()
-
-    def passed(self, parity):            # mbarrier.try_wait.parity: true once the phase with this parity has completed
-        return self.phase != parity
-
-
-def _simulate_pair_protocol(seed, npairs_total, nclusters, units, AS, BS):
-    import random
-    rnd = random.Random(seed)
-    A_BYTES, B_HALF = 20480, 8192
-    EPI_WARPS = 8
-    log = []
-
-    class CTA:
-        def __init__(self):
-            self.full_b = [_MBar(1) for _ in range(BS)]; self.empty_b = [_MBar(1) for _ in range(BS)]
-            self.full_a = [_MBar(1) for _ in range(AS)]; self.empty_a = [_MBar(1) for _ in range(AS)]
-            self.tm_full = [_MBar(1) for _ in range(2)]; self.tm_empty = [_MBar(2 * EPI_WARPS) for _ in range(2)]
-            self.a = [None] * AS; self.b = [None] * BS          # stage contents (tags); None = never written
-            self.a_busy = [0] * AS; self.b_busy = [0] * BS      # MMAs issued on the stage and not yet completed
-            self.acc = [None, None]                             # accumulator tag per TMEM stage
-            self.acc_unread = [0, 0]                            # epilogue warps that still have to read the stage
-
-    for cid in range(nclusters):
-        ctas = [CTA(), CTA()]
-        leader = ctas[0]
-        events = []                                             # (time, seq, fn): asynchronous completions
-        now = [0]; seq = [0]
-
-        def later(fn, lo=1, hi=40):
-            seq[0] += 1
-            events.append((now[0] + rnd.randint(lo, hi), seq[0], fn))
-
-        pairs = list(range(cid, npairs_total, nclusters))
-
-        def producer(rank):
-            me = ctas[rank]
-            ia = ib = 0
-
-            def load_a(tag):
-                nonlocal ia
-                sa, pa = ia % AS, (ia // AS) & 1
-                while not me.empty_a[sa].passed(pa ^ 1):
-                    yield
-                if rank == 0:
-                    leader.full_a[sa].arrive(tx=2 * A_BYTES)
-
-                def done(sa=sa, tag=tag):
-                    assert me.a_busy[sa] == 0, "A stage overwritten while an MMA may still read it"
-                    me.a[sa] = tag
-                    leader.full_a[sa].complete_tx(A_BYTES)       # .cta_group::2: completes on the LEADER's barrier
-                later(done)
-                ia += 1
-            for pair in pairs:
-                yield from load_a((pair, 0, rank))
-                for u in range(units):
-                    if u + 1 < units:
-                        yield from load_a((pair, u + 1, rank))
-                    for dy in range(3):
-                        sb, pb = ib % BS, (ib // BS) & 1
-                        while not me.empty_b[sb].passed(pb ^ 1):
-                            yield
-                        if rank == 0:
-                            leader.full_b[sb].arrive(tx=2 * B_HALF)
-
-                        def done(sb=sb, tag=(pair, u, dy, rank)):
-                            assert me.b_busy[sb] == 0, "B stage overwritten while an MMA may still read it"
-                            me.b[sb] = tag
-                            leader.full_b[sb].complete_tx(B_HALF)
-                        later(done)
-                        ib += 1
-                        yield
-
-        def mma():
-            it = ia = tcount = 0
-            for pair in pairs:
-                acs, aph = tcount & 1, (tcount >> 1) & 1
-                while not leader.tm_empty[acs].passed(aph ^ 1):
-                    yield
-                for c in ctas:
-                    assert c.acc_unread[acs] == 0, "accumulator stage overwritten before its epilogue finished"
-                for u in range(units):
-                    sa, pa = ia % AS, (ia // AS) & 1
-                    while not leader.full_a[sa].passed(pa):
-                        yield
-                    for dy in range(3):
-                        sb, pb = it % BS, (it // BS) & 1
-                        while not leader.full_b[sb].passed(pb):
-                            yield
-                        for r, c in enumerate(ctas):             # one MMA reads both CTAs' stages
-                            assert c.a[sa] == (pair, u, r), (c.a[sa], pair, u, r)
-                            assert c.b[sb] == (pair, u, dy, r), (c.b[sb], pair, u, dy, r)
-                            c.a_busy[sa] += 1; c.b_busy[sb] += 1
-                            if u == 0 and dy == 0:
-                                c.acc[acs] = [pair, 0]           # accumulate flag 0: overwrite
-                            assert c.acc[acs][0] == pair
-                            c.acc[acs][1] += 1
-
-                        def b_done(sa=sa, sb=sb):                # commit: arrives once the MMAs issued so far completed
-                            for c in ctas:
-                                c.b_busy[sb] -= 1; c.a_busy[sa] -= 1
-                                c.empty_b[sb].arrive()           # multicast to both CTAs
-                        later(b_done, 5, 30)
-                        it += 1
-                        yield
-
-                    def a_done(sa=sa):
-                        for c in ctas:
-                            c.empty_a[sa].arrive()
-                    later(a_done, 31, 45)                        # after the MMAs' own completions (commit order)
-                    ia += 1
-
-                def full(acs=acs):
-                    for c in ctas:
-                        c.acc_unread[acs] = EPI_WARPS
-                        c.tm_full[acs].arrive()
-                later(full, 46, 60)
-                tcount += 1
-
-        def epilogue_warp(rank, w):
-            me = ctas[rank]
-            tcount = 0
-            for pair in pairs:
-                acs, aph = tcount & 1, (tcount >> 1) & 1
-                while not me.tm_full[acs].passed(aph):
-                    yield
-                assert me.acc[acs] == [pair, units * 3], (me.acc[acs], pair)
-                for _ in range(rnd.randint(0, 3)):
-                    yield
-                me.acc_unread[acs] -= 1
-                leader.tm_empty[acs].arrive()                    # remote arrive on the leader's barrier
-                log.append((cid, pair, rank, w))
-                tcount += 1
-                yield
-
-        actors = [producer(0), producer(1), mma()] + [epilogue_warp(r, w) for r in range(2) for w in range(EPI_WARPS)]
-        alive = list(actors)
-        idle_rounds = 0
-        while alive:
-            now[0] += 1
-            due = sorted(e for e in events if e[0] <= now[0])
-            for e in due:
-                events.remove(e)
-                e[2]()
-            progressed = bool(due)
-            rnd.shuffle(alive)
-            for a in list(alive):
-                if rnd.random() < 0.6:
-                    try:
-                        next(a)
-                    except StopIteration:
-                        alive.remove(a)
-                    progressed = True
-            idle_rounds = 0 if (progressed or events) else idle_rounds + 1
-            assert now[0] < 2_000_000 and idle_rounds < 50, "deadlock"
-        while events:                                            # drain completions after the last actor left
-            events.sort()
-            events.pop(0)[2]()
-    return log
-
-
-def test_cta_pair_convolution_protocol_emulation():
-    for seed, (npairs, nclusters, units) in enumerate([(7, 2, 6), (5, 5, 3), (9, 4, 21), (1, 1, 3), (12, 3, 9)]):
-        log = _simulate_pair_protocol(seed, npairs, nclusters, units, AS=3, BS=12 if seed % 2 else 6)
-        done = {(pair, rank) for _, pair, rank, _ in log}
-        assert done == {(p, r) for p in range(npairs) for r in range(2)}
-        assert len(log) == npairs * 2 * 8
-
-
 def test_forward_placeholders_are_not_none():
     """RaftVisualFrontend.forward returns empty, non-None x0 / factors like the reference's empty gtsam containers
     (visual_frontend.py:248-249): the reference's VioSLAM._frontend stops the pipeline on `x0 is None`
@@ -321,76 +128,3 @@ def test_forward_placeholders_are_not_none():
     from nerf_slam_b200.frontend import EmptyFactorGraph, EmptyValues
     x0, f = EmptyValues(), EmptyFactorGraph()
     assert x0 is not None and f is not None and bool(x0) and x0.size() == 0 and len(f) == 0
-
-
-def test_cta_pair_operand_addressing_reproduces_the_convolution():
-    """data-path emulation of csrc/conv_igemm2.cu: CTA rank r of pair p computes tile 2p + r; the weight block of
-    (tap, channel block) is fetched as two 2-D boxes {64, N/2} at rows blk*N + r*N/2 of the packed image viewed as
-    [blocks*N, 64] (no TMA swizzle: the image already is the swizzled smem layout); one MMA of the pair multiplies each
-    CTA's 128 pixel rows with the N columns formed by CTA 0's half (columns 0..N/2-1) and CTA 1's half (N/2..N-1).
-    An odd tile count leaves rank 1 of the last pair with an out-of-range tile (zero-filled loads, clipped stores)."""
-    import torch.nn.functional as F
-    from nerf_slam_b200.conv import pack_weights
-    g = torch.Generator().manual_seed(11)
-    B, H, W, N = 1, 20, 40, 128                                 # 3 x 3 = 9 tiles -> 5 pairs, the last one half empty
-    chans = [64, 40]
-    srcs = [torch.randn(B, H, W, c, generator=g) for c in chans]
-    w = torch.randn(N, sum(chans), 3, 3, generator=g) * 0.1
-    image = pack_weights(w, chans).float().view(-1, 64)         # the 2-D tensor the weight tensor map describes
-    cbs = [(c + 63) // 64 for c in chans]
-    cb_total = sum(cbs)
-    assert image.shape[0] == 9 * cb_total * N
-    rows = torch.arange(N // 2)
-
-    def half_block(blk, rank):                                  # box {64, N/2} at row blk*N + rank*N/2, then un-swizzle
-        box = image[blk * N + rank * (N // 2): blk * N + (rank + 1) * (N // 2)].view(N // 2, 8, 8)
-        out = torch.empty(N // 2, 8, 8)
-        for j in range(8):
-            out[rows, j] = box[rows, j ^ (rows & 7)]            # row phase = (row within the half) & 7 == (row in block) & 7
-        return out.reshape(N // 2, 64)
-
-    ref = F.conv2d(torch.cat(srcs, -1).permute(0, 3, 1, 2).half().float(), w.half().float(), padding=1).permute(0, 2, 3, 1)
-    got = torch.full((B, H, W, N), float("nan"))
-    TH, TW = 8, 16
-    tiles_h, tiles_w = (H + TH - 1) // TH, (W + TW - 1) // TW
-    ntiles = B * tiles_h * tiles_w
-    assert ntiles % 2 == 1
-    for pair in range((ntiles + 1) // 2):
-        acc = [torch.zeros(TH * TW, N), torch.zeros(TH * TW, N)]
-        geo = []
-        for rank in range(2):
-            tile = 2 * pair + rank
-            n, tt = tile // (tiles_h * tiles_w), tile % (tiles_h * tiles_w)
-            geo.append((tile, n, (tt // tiles_w) * TH, (tt % tiles_w) * TW))
-        cbg = 0
-        for s, c in enumerate(chans):
-            for cb in range(cbs[s]):
-                for dx in range(3):
-                    tiles = []
-                    for rank in range(2):
-                        tile, n, h0, w0 = geo[rank]
-                        t = torch.zeros(TH + 2, TW, 64)
-                        for hy in range(TH + 2):
-                            for wx in range(TW):
-                                y, x = h0 - 1 + hy, w0 + dx - 1 + wx
-                                if n < B and 0 <= y < H and 0 <= x < W:      # image index B: everything out of range
-                                    ce = min(c, cb * 64 + 64)
-                                    t[hy, wx, :ce - cb * 64] = srcs[s][n, y, x, cb * 64:ce].half().float()
-                        tiles.append(t.reshape(-1, 64))
-                    for dy in range(3):
-                        blk = (dy * 3 + dx) * cb_total + cbg
-                        Bfull = torch.cat([half_block(blk, 0), half_block(blk, 1)], 0)     # [N, 64]: CTA 0's half first
-                        for rank in range(2):
-                            acc[rank] += tiles[rank][dy * TW:dy * TW + TH * TW] @ Bfull.T
-                cbg += 1
-        for rank in range(2):
-            tile, n, h0, w0 = geo[rank]
-            if tile >= ntiles:
-                assert float(acc[rank].abs().max()) == 0.0           # nothing but zero fill reached the missing tile
-                continue
-            for r in range(TH * TW):
-                y, x = h0 + r // TW, w0 + r % TW
-                if y < H and x < W:
-                    got[n, y, x] = acc[rank][r]
-    assert not torch.isnan(got).any()
-    assert float((got - ref).abs().max()) < 2e-3

@@ -112,7 +112,7 @@ def _worker(rank, world, port, q):
         q.put((rank, traceback.format_exc()))
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_two_rank_nccl_gradients_equal_single_process_and_handoff_is_exact():
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")

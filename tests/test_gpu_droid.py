@@ -21,7 +21,7 @@ def _net():
 
 
 def test_update_net_reference_convention_matches_library():
-    """UpdateNetTC (tcgen05) vs the library-convolution UpdateModule on the reference's tensor layouts;
+    """UpdateNetTC (wgmma) vs the library-convolution UpdateModule on the reference's tensor layouts;
     tolerances of tests/test_gpu_conv.py (fp16 operands, different summation order)"""
     net = _net()
     g = torch.Generator(device=DEV).manual_seed(5)

@@ -1,4 +1,4 @@
-"""GPU parity tests: hand-written sm_100a kernels (through the C ABI) vs the CPU oracle on the same
+"""GPU parity tests: hand-written sm_90a kernels (through the C ABI) vs the CPU oracle on the same
 seeded inputs.  Tolerances are stated per test (SURVEY.md §8c / north_star: bit-exact for the
 fp16 lookup and integer work, fp32 tolerances elsewhere)."""
 import os

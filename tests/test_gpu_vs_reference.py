@@ -1,4 +1,4 @@
-"""GPU parity against the REFERENCE'S OWN CUDA kernels, compiled for sm_100a from /root/reference
+"""GPU parity against the REFERENCE'S OWN CUDA kernels, compiled for sm_90a from /root/reference
 by oracle/build_ref.py into oracle/_ref/*.so (shipped to the GPU box; skipped if absent).
 This is what pins the parity claim: same seeded inputs through both implementations."""
 import numpy as np
