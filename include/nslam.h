@@ -111,6 +111,28 @@ int nslam_tsdf_integrate(float* tsdf, float* weight, float* color, int nx, int n
                          int H, int W, const float* intr4_host, const float* cam_T_world_tq, float max_depth,
                          float sdf_trunc, float max_weight, float max_depth_sigma, void* stream);
 
+/* Read-outs of that volume (csrc/tsdf_mesh.cu; TsdfFusion.build_mesh / render_volume, reference :556-573, :319-484).
+ * Marching cubes in three calls: _plan -> int32 scratch size (cudaErrorInvalidValue when the grid's worst-case vertex or
+ * triangle count overflows int32); _count -> scratch[0..2] = vertices, triangles, active voxels (DEVICE); _emit with the
+ * same volume and min_weight -> active [A,4] int32 scratch, vertices / vertex_colors ([0,1]) / vertex_normals [V,3] fp32,
+ * triangles [T,3] int32 in a fixed order (vertices by owning voxel then axis, triangles by cube then table order).
+ * A cube is meshed when its 8 corners have weight > min_weight.  origin3 (HOST) as above. */
+int nslam_tsdf_mesh_plan(int nx, int ny, int nz, long long* scratch_ints);
+int nslam_tsdf_mesh_count(const float* tsdf, const float* weight, int nx, int ny, int nz, float min_weight, int* scratch,
+                          void* stream);
+int nslam_tsdf_mesh_emit(const float* tsdf, const float* weight, const float* color, int nx, int ny, int nz,
+                         const float* origin3_host, float voxel_size, float min_weight, const int* scratch, int n_active,
+                         int* active, float* vertices, float* vertex_colors, float* vertex_normals, int* triangles,
+                         void* stream);
+/* Ray cast n views in one launch: cam_T_world_tq [n,7] (DEVICE, the packet's poses), intr4 = fx, fy, cx, cy (HOST);
+ * z-depth march from min_depth to max_depth, hit = first + -> - transition of the trilinear TSDF between samples whose
+ * 8 corners have weight > min_weight.  depth [n,H,W] (0 = miss), color [n,H,W,3] in [0,1], weight [n,H,W], normal
+ * [n,H,W,3] or NULL (DEVICE). */
+int nslam_tsdf_raycast(const float* tsdf, const float* weight, const float* color, int nx, int ny, int nz,
+                       const float* origin3_host, float voxel_size, const float* cam_T_world_tq, int n, int H, int W,
+                       const float* intr4_host, float min_depth, float max_depth, float sdf_trunc, float min_weight,
+                       float* depth, float* color_out, float* weight_out, float* normal_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
