@@ -22,6 +22,12 @@ extern "C" {
 int nslam_corr_index_forward(const void* volume, int dtype, const float* coords, void* out, int n,
                              int h1, int w1, int h2, int w2, int radius, void* stream);
 
+/* droid_backends.corr_index_backward (src/droid.cpp:290-301; kernel src/correlation_kernels.cu:73-124, host :157-185)
+ * coords [n,2,h1,w1] fp32, corr_grad [n,2r+1,2r+1,h1,w1] and volume_grad [n,h1,w1,h2,w2] in `dtype` (0 fp16, 1 fp32).
+ * Every element of volume_grad is written (zeros outside the windows); volume_grad must be 16-byte aligned. */
+int nslam_corr_index_backward(const float* coords, const void* corr_grad, int dtype, void* volume_grad, int n, int h1,
+                              int w1, int h2, int w2, int radius, void* stream);
+
 /* CorrBlock.__call__ (networks/modules/corr.py:40-50) fused over the pyramid:
  * volumes: HOST array of num_levels device pointers, h2s/w2s: HOST int arrays;
  * coords [n,2,h1,w1] in level-0 pixels (level l samples coords/2^l); out [n,L*(2r+1)^2,h1,w1].
@@ -61,6 +67,18 @@ int nslam_corr_volume_build_slots(const void* fmaps, int NF, int H, int W, int C
 int nslam_altcorr_forward(const void* fmap1, const void* fmap2, int dtype, const float* coords,
                           void* corr, int B, int N, int H1, int W1, int H2, int W2, int C,
                           int radius, void* stream);
+
+/* droid_backends.altcorr_backward (src/droid.cpp:315-327; kernel src/altcorr_kernel.cu:152-286, host :321-356), fp32:
+ * fmap1 [B,H1,W1,C], fmap2 [B,H2,W2,C], coords [B,N,H1,W1,2], corr_grad [B,N,(2r+1)^2,H1,W1] ->
+ * fmap1_grad [B,H1,W1,C], fmap2_grad [B,H2,W2,C], both fully written.  Deterministic: no float atomics, the scatter
+ * into fmap2_grad goes through bucket lists in `scratch` (DEVICE, at least the bytes that
+ * nslam_altcorr_backward_scratch returns for the same shapes).  C % 4 == 0, C <= 512, 1 <= r <= 4.
+ * The coordinate gradient is not computed (the reference returns zeros). */
+int nslam_altcorr_backward_scratch(int B, int N, int H1, int W1, int H2, int W2, int C, int radius,
+                                   unsigned long long* bytes);
+int nslam_altcorr_backward(const float* fmap1, const float* fmap2, const float* coords, const float* corr_grad,
+                           float* fmap1_grad, float* fmap2_grad, void* scratch, unsigned long long scratch_bytes, int B,
+                           int N, int H1, int W1, int H2, int W2, int C, int radius, void* stream);
 
 /* pops.projective_transform, jacobian=False (networks/geom/projective_ops.py:98-145) as used by
  * RaftVisualFrontend.reproject (slam/visual_frontends/visual_frontend.py:909-918).

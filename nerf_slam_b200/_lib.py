@@ -57,6 +57,10 @@ _SIGNATURES = {
     "nslam_corr_volume_build_slots": [_P, c_int, c_int, c_int, c_int, _P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P],
     "nslam_corr_volume_build_simt": [_P, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, _P, _P, _P, _P],
     "nslam_altcorr_forward": [_P, _P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P],
+    "nslam_corr_index_backward": [_P, _P, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P],
+    "nslam_altcorr_backward_scratch": [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P],
+    "nslam_altcorr_backward": [_P, _P, _P, _P, _P, _P, _P, ctypes.c_ulonglong, c_int, c_int, c_int, c_int, c_int, c_int,
+                               c_int, c_int, _P],
     "nslam_reproject": [_P, _P, _P, c_int, _P, _P, c_int, c_int, c_int, _P, _P, _P],
     "nslam_frame_distance": [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_float, _P, _P],
     "nslam_projmap": [_P, _P, _P, _P, _P, c_int, c_int, c_int, _P, _P, _P],

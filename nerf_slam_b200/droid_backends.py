@@ -2,7 +2,8 @@
 
 Same 12 function names, argument order, tensor layouts, in-place semantics and error behaviour
 as the pybind module defined at reference src/droid.cpp:347-363 — but every function forwards to
-a hand-written sm_90a kernel through the C ABI of libnslam_sm90a.so (include/nslam.h).
+a hand-written sm_90a kernel through the C ABI of libnslam_sm90a.so (include/nslam.h), the two
+training-only backward operators (corr_index_backward, altcorr_backward) included.
 `import nerf_slam_b200.droid_backends as droid_backends` (or put `nerf_slam_b200/shim` on
 sys.path) and the reference's networks/modules/corr.py + visual_frontend.py run unchanged.
 
@@ -74,10 +75,22 @@ def corr_index_forward(volume, coords, radius):
 
 
 def corr_index_backward(volume, coords, corr_grad, radius):
-    """src/droid.cpp:290-301. Training only; the inference path runs with autograd disabled
-    (examples/slam_demo.py:198).  Symbol kept; out of scope of the hot path (SURVEY.md §2.2)."""
-    raise NotImplementedError("corr_index_backward: training-only operator, not part of the "
-                              "inference hot path (SURVEY.md §8, out of scope)")
+    """src/droid.cpp:290-301 -> [volume_grad] (shape and dtype of `volume`).  Training only: the SLAM path runs with
+    autograd disabled.  Bit-exact w.r.t. the reference kernel in fp16 and fp32 (csrc/corr_backward.cu)."""
+    _chk(volume, coords, corr_grad)
+    lib = _lib.load()
+    n, h1, w1, h2, w2 = volume.shape
+    if volume.dtype not in _DT or corr_grad.dtype != volume.dtype:
+        raise RuntimeError("corr_index_backward: fp16/fp32 volumes only, corr_grad in the volume's dtype")
+    rd = 2 * radius + 1
+    if tuple(corr_grad.shape) != (n, rd, rd, h1, w1) or tuple(coords.shape) != (n, 2, h1, w1):
+        raise RuntimeError("corr_index_backward: shape mismatch")
+    coords = coords.float().contiguous()
+    grad = torch.empty_like(volume)
+    _lib.check(lib.nslam_corr_index_backward(_lib.ptr(coords), _lib.ptr(corr_grad), _DT[volume.dtype],
+                                             _lib.ptr(grad), n, h1, w1, h2, w2, radius, _lib.stream_ptr()),
+               "corr_index_backward")
+    return [grad]
 
 
 def corr_lookup_pyramid(volumes, coords, radius, slots=None, nhwc_stride=0, coords_nhwc=False, out=None):
@@ -161,8 +174,30 @@ def altcorr_forward(fmap1, fmap2, coords, radius):
 
 
 def altcorr_backward(fmap1, fmap2, coords, corr_grad, radius):
-    """src/droid.cpp:315-327. Training only (see corr_index_backward)."""
-    raise NotImplementedError("altcorr_backward: training-only operator, out of scope")
+    """src/droid.cpp:315-327 -> [fmap1_grad, fmap2_grad, coords_grad].  fp32 only, like the reference.
+    coords_grad is all zeros: the reference allocates it with zeros and its kernel never writes it.
+    Deterministic: the fmap2 scatter is laid out by bucket lists instead of float atomics (csrc/corr_backward.cu)."""
+    _chk(fmap1, fmap2, coords, corr_grad)
+    lib = _lib.load()
+    if any(t.dtype != torch.float32 for t in (fmap1, fmap2, coords, corr_grad)):
+        raise RuntimeError("altcorr_backward: fp32 tensors only")
+    B, H1, W1, C = fmap1.shape
+    _, H2, W2, _ = fmap2.shape
+    N = coords.shape[1]
+    rd = 2 * radius + 1
+    if (fmap2.shape[0] != B or fmap2.shape[3] != C or tuple(coords.shape) != (B, N, H1, W1, 2)
+            or tuple(corr_grad.shape) != (B, N, rd * rd, H1, W1)):
+        raise RuntimeError("altcorr_backward: shape mismatch")
+    nbytes = ctypes.c_ulonglong(0)
+    _lib.check(lib.nslam_altcorr_backward_scratch(B, N, H1, W1, H2, W2, C, radius, ctypes.byref(nbytes)),
+               "altcorr_backward (unsupported shape)")
+    scratch = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=fmap1.device)
+    g1 = torch.empty_like(fmap1)
+    g2 = torch.empty_like(fmap2)
+    _lib.check(lib.nslam_altcorr_backward(_lib.ptr(fmap1), _lib.ptr(fmap2), _lib.ptr(coords), _lib.ptr(corr_grad),
+                                          _lib.ptr(g1), _lib.ptr(g2), _lib.ptr(scratch), nbytes.value, B, N, H1, W1,
+                                          H2, W2, C, radius, _lib.stream_ptr()), "altcorr_backward")
+    return [g1, g2, torch.zeros_like(coords)]
 
 
 # ------------------------------------------------------------------------------------------ geometry
