@@ -42,6 +42,9 @@ def parse_args(argv=None):
     p.add_argument("--height", "--screenshot_h", type=int, default=0, help="Resolution height of GUI and screenshots.")
     p.add_argument("--network", default="", help="Path to the network config. Uses the scene's default if unspecified.")
     p.add_argument("--eval", action="store_true", help="Evaluate method.")
+    p.add_argument("--tsdf_volume", type=str, default="dense", choices=["dense", "blocks"],
+                   help="--fusion=tsdf/sigma volume: a dense grid, or unbounded 16^3 voxel blocks allocated where depth reaches")
+    p.add_argument("--tsdf_block_count", type=int, default=5000, help="initial block capacity of --tsdf_volume=blocks")
     # additions (not in the reference): bounds for a non-interactive run
     p.add_argument("--synthetic_frames", type=int, default=200, help="frames of the procedural stream (--dataset_dir=synthetic)")
     p.add_argument("--nerf_iters_per_frame", type=int, default=2, help="NeRF training steps interleaved per input frame")

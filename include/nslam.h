@@ -151,6 +151,43 @@ int nslam_tsdf_raycast(const float* tsdf, const float* weight, const float* colo
                        const float* intr4_host, float min_depth, float max_depth, float sdf_trunc, float min_weight,
                        float* depth, float* color_out, float* weight_out, float* normal_out, void* stream);
 
+/* §8(f3) sparse voxel-block volume (csrc/tsdf_blocks.cu; semantics at its head): 16^3 blocks allocated where the depth
+ * maps reach, a pool [B,16,16,16] (tsdf, weight fp32, colour x3 fp32) in a fixed order, an open-addressing hash table
+ * of block keys (int64, -1 = empty; capacity a power of two, load <= 1/2).  Per keyframe: _activate (one pinned read of
+ * the touched / new block counts) -> _insert (or _rehash into a larger table) -> _integrate.  Read-outs: _neighbours
+ * [B,27] -> _mesh_plan / _mesh_count / _mesh_emit (csrc/tsdf_mesh.cu) and _raycast, equal to the dense read-outs of
+ * the volume's dense embedding at lattice origin 0. */
+int nslam_tsdf_blocks_scratch(int H, int W, long long* bytes);
+int nslam_tsdf_blocks_activate(const float* idepth_up, const float* depth_cov_up, int H, int W, const float* intr4_host,
+                               const float* cam_T_world_tq, float voxel_size, float max_depth, float max_depth_sigma,
+                               const long long* hash_keys, const int* hash_vals, int hash_cap, int n_blocks, void* scratch,
+                               long long scratch_bytes, int* touched, long long* new_keys, int* counts_dev,
+                               int* counts_host, void* stream);
+int nslam_tsdf_blocks_insert(const long long* new_keys, int n_new, int n_blocks, long long* pool_keys, int* pool_coords,
+                             float* tsdf, float* weight, float* color, long long* hash_keys, int* hash_vals, int hash_cap,
+                             void* stream);
+int nslam_tsdf_blocks_rehash(const long long* pool_keys, int n_blocks, long long* hash_keys, int* hash_vals, int hash_cap,
+                             void* stream);
+int nslam_tsdf_blocks_integrate(float* tsdf, float* weight, float* color, const int* pool_coords, const int* touched,
+                                int n_touched, float voxel_size, const float* idepth_up, const float* depth_cov_up,
+                                const unsigned char* rgb_chw, int H, int W, const float* intr4_host,
+                                const float* cam_T_world_tq, float max_depth, float sdf_trunc, float max_weight,
+                                float max_depth_sigma, void* stream);
+int nslam_tsdf_blocks_neighbours(const int* pool_coords, int n_blocks, const long long* hash_keys, const int* hash_vals,
+                                 int hash_cap, int* neighbours, void* stream);
+int nslam_tsdf_blocks_mesh_plan(int n_blocks, long long* scratch_ints);
+int nslam_tsdf_blocks_mesh_count(const float* tsdf, const float* weight, const int* neighbours, const int* block_coords,
+                                 int n_blocks, float min_weight, int* scratch, void* stream);
+int nslam_tsdf_blocks_mesh_emit(const float* tsdf, const float* weight, const float* color, const int* neighbours,
+                                const int* block_coords, int n_blocks, float voxel_size, float min_weight, const int* scratch,
+                                int n_active, int* active, float* vertices, float* vertex_colors, float* vertex_normals,
+                                int* triangles, void* stream);
+int nslam_tsdf_blocks_raycast(const float* tsdf, const float* weight, const float* color, const int* neighbours,
+                              const long long* hash_keys, const int* hash_vals, int hash_cap, float voxel_size,
+                              const float* cam_T_world_tq, int n, int H, int W, const float* intr4_host, float min_depth,
+                              float max_depth, float sdf_trunc, float min_weight, float* depth, float* color_out,
+                              float* weight_out, float* normal_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -85,6 +85,19 @@ _SIGNATURES = {
     "nslam_tsdf_mesh_emit": [_P, _P, _P, c_int, c_int, c_int, _P, c_float, c_float, _P, c_int, _P, _P, _P, _P, _P, _P],
     "nslam_tsdf_raycast": [_P, _P, _P, c_int, c_int, c_int, _P, c_float, _P, c_int, c_int, c_int, _P, c_float, c_float,
                            c_float, c_float, _P, _P, _P, _P, _P],
+    "nslam_tsdf_blocks_scratch": [c_int, c_int, _P],
+    "nslam_tsdf_blocks_activate": [_P, _P, c_int, c_int, _P, _P, c_float, c_float, c_float, _P, _P, c_int, c_int, _P,
+                                   ctypes.c_longlong, _P, _P, _P, _P, _P],
+    "nslam_tsdf_blocks_insert": [_P, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, c_int, _P],
+    "nslam_tsdf_blocks_rehash": [_P, c_int, _P, _P, c_int, _P],
+    "nslam_tsdf_blocks_integrate": [_P, _P, _P, _P, _P, c_int, c_float, _P, _P, _P, c_int, c_int, _P, _P, c_float, c_float,
+                                    c_float, c_float, _P],
+    "nslam_tsdf_blocks_neighbours": [_P, c_int, _P, _P, c_int, _P, _P],
+    "nslam_tsdf_blocks_mesh_plan": [c_int, _P],
+    "nslam_tsdf_blocks_mesh_count": [_P, _P, _P, _P, c_int, c_float, _P, _P],
+    "nslam_tsdf_blocks_mesh_emit": [_P, _P, _P, _P, _P, c_int, c_float, c_float, _P, c_int, _P, _P, _P, _P, _P, _P],
+    "nslam_tsdf_blocks_raycast": [_P, _P, _P, _P, _P, _P, c_int, c_float, _P, c_int, c_int, c_int, _P, c_float, c_float,
+                                  c_float, c_float, _P, _P, _P, _P, _P],
     "nslam_ba_reduced_camera_matrix": [ctypes.POINTER(BAGraph), ctypes.POINTER(BABuffers), _P],
     "nslam_ba_tile_pixels": [],
     "nslam_ba_solve": [_P, _P, c_int, c_int, _P, c_float, c_float, c_float, _P, _P, _P, _P, _P],

@@ -18,8 +18,10 @@
 // depth mask are evaluated on the fly from the packet's tensors (the reference materialises three images per frame).
 // The set of updated voxels is every grid voxel that passes the reference's own tests (a superset of its activated
 // blocks: voxels far in front of the surface receive the saturated value +1 there only if their block was activated).
+// The sparse voxel-block volume (tsdf_blocks.cu) updates exactly the activated blocks instead; both share the per-voxel
+// rule of tsdf_rules.cuh.
 // HBM-bound: 20 B read + 20 B written per voxel inside the frustum, 4 B otherwise.
-#include "common.cuh"
+#include "tsdf_rules.cuh"
 
 namespace nslam {
 
@@ -32,26 +34,11 @@ struct TsdfGrid {
   float voxel;
 };
 
-struct TsdfFrame {
-  const float* idepth;      // [H,W] inverse depth (upsampled)
-  const float* depth_cov;   // [H,W] depth variance, or NULL = uniform weight 1
-  const unsigned char* rgb; // [3,H,W] u8
-  int H, W;
-  float fx, fy, cx, cy;
-  const float* pose;        // cam_T_world [t, q_xyzw] on the DEVICE (x_cam = R(q) x_world + t): no host copy of the pose
-  float max_depth, trunc, max_weight, max_sigma;
-};
-
 __global__ void __launch_bounds__(256)
 tsdf_integrate_kernel(TsdfGrid g, TsdfFrame f) {
   __shared__ double sR[9], st[3];
   if (threadIdx.x == 0) {
-    // SE3(poses).matrix() is a float32 matrix that build_volume promotes to float64 (:186, :209): round the rotation to fp32
-    const double qx = f.pose[3], qy = f.pose[4], qz = f.pose[5], qw = f.pose[6];
-    const double R[9] = {1 - 2 * (qy * qy + qz * qz), 2 * (qx * qy - qz * qw), 2 * (qx * qz + qy * qw),
-                         2 * (qx * qy + qz * qw), 1 - 2 * (qx * qx + qz * qz), 2 * (qy * qz - qx * qw),
-                         2 * (qx * qz - qy * qw), 2 * (qy * qz + qx * qw), 1 - 2 * (qx * qx + qy * qy)};
-    for (int i = 0; i < 9; i++) sR[i] = (double)(float)R[i];
+    tsdf_pose_rotation(f.pose, sR);
     st[0] = f.pose[0]; st[1] = f.pose[1]; st[2] = f.pose[2];
   }
   __syncthreads();
@@ -60,38 +47,9 @@ tsdf_integrate_kernel(TsdfGrid g, TsdfFrame f) {
   if (ix >= g.nx) return;
   // the reference's voxel coordinates are float32 tensors (metric: voxel_size * index, lattice through `origin`), promoted to
   // float64 together with extrinsic and intrinsic for the projection (:243-252): float32 product, float32 sum, no contraction
-  const double wx = (double)__fadd_rn(__fmul_rn(g.voxel, (float)ix), g.ox), wy = (double)__fadd_rn(__fmul_rn(g.voxel, (float)iy), g.oy),
-               wz = (double)__fadd_rn(__fmul_rn(g.voxel, (float)iz), g.oz);
-  const double x = sR[0] * wx + sR[1] * wy + sR[2] * wz + st[0];
-  const double y = sR[3] * wx + sR[4] * wy + sR[5] * wz + st[1];
-  const double d = sR[6] * wx + sR[7] * wy + sR[8] * wz + st[2];
-  if (!(d > 0.0)) return;
-  const long long u = llrint(((double)f.fx * x + (double)f.cx * d) / d);     // round-half-even, like Tensor.round()
-  const long long v = llrint(((double)f.fy * y + (double)f.cy * d) / d);
-  if (u < 0 || v < 0 || u >= f.W || v >= f.H) return;
-  const size_t pix = (size_t)v * f.W + (size_t)u;
-  float depth = 1.0f / f.idepth[pix];
-  float wr = 1.0f;
-  if (f.depth_cov) {
-    const float cov = f.depth_cov[pix];
-    wr = sqrtf(1.0f / cov);                                   // cov.pow(-1).sqrt()  (:196)
-    if (!(sqrtf(cov) < f.max_sigma)) depth = f.max_depth + 1.0f;   // masked pixels are pushed beyond max_depth (:201-203, :549)
-  }
-  float sdf = depth - (float)d;
-  if (!(depth > 0.f && depth < f.max_depth && sdf >= -f.trunc)) return;
-  sdf = fminf(sdf, f.trunc) / f.trunc;
   const size_t vi = ((size_t)iz * g.ny + iy) * g.nx + ix;
-  const float w = g.weight[vi];
-  const float wp = w + wr;
-  // products and sum rounded separately, like the tensor expression (:280-281) — no FMA contraction
-  g.tsdf[vi] = __fdiv_rn(__fadd_rn(__fmul_rn(w, g.tsdf[vi]), __fmul_rn(wr, sdf)), wp);
-  const size_t hw = (size_t)f.H * f.W;
-#pragma unroll
-  for (int c = 0; c < 3; c++) {
-    const float col = (float)f.rgb[(size_t)c * hw + pix];
-    g.color[vi * 3 + c] = __fdiv_rn(__fadd_rn(__fmul_rn(w, g.color[vi * 3 + c]), __fmul_rn(wr, col)), wp);
-  }
-  g.weight[vi] = fminf(wp, f.max_weight);
+  tsdf_update_voxel(f, sR, st, __fadd_rn(__fmul_rn(g.voxel, (float)ix), g.ox), __fadd_rn(__fmul_rn(g.voxel, (float)iy), g.oy),
+                    __fadd_rn(__fmul_rn(g.voxel, (float)iz), g.oz), g.tsdf + vi, g.weight + vi, g.color + vi * 3);
 }
 
 }  // namespace nslam

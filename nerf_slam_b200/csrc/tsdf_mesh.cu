@@ -23,7 +23,7 @@
 // frame, z-depth) from min_depth to max_depth through the trilinear TSDF.  A sample is observed when its 8 cell corners have
 // weight > min_weight.  Steps along the ray: voxel while unobserved or not in front of the surface, max(f * sdf_trunc, voxel)
 // in front of it.  The hit is the first + -> (<= 0) transition between consecutive observed samples, linearly interpolated.
-#include "common.cuh"
+#include "tsdf_rules.cuh"
 
 #include <climits>
 
@@ -108,12 +108,79 @@ constexpr int kMeshBlock = 256;
 constexpr int kScanThreads = 1024;
 constexpr int kScanItems = 4;          // block counts per scan thread per chunk
 
-struct MeshVolume {
+// Voxel accessors of the two volumes.  The passes below address voxels by accessor coordinates (i,j,k) relative to a
+// voxel bound with `bind`, read tsdf / weight / colour there, and ask whether a voxel exists (`inside`: the dense grid has
+// borders, the block volume has none — its unallocated voxels read as tsdf 0, weight 0, colour 0).  `pos` gives the
+// lattice index a vertex position is formed from.
+
+// dense grid [nz,ny,nx]: accessor coordinates are grid indices, records keyed by the linear voxel index
+struct DenseVox {
   const float* tsdf;
   const float* weight;
   const float* color;
   int nx, ny, nz;
-  float min_weight;
+  __device__ __forceinline__ size_t idx(int i, int j, int k) const { return ((size_t)k * ny + j) * nx + i; }
+  __device__ __forceinline__ bool inside(int i, int j, int k) const {
+    return i >= 0 && j >= 0 && k >= 0 && i < nx && j < ny && k < nz;
+  }
+  __device__ __forceinline__ float t(int i, int j, int k) const { return tsdf[idx(i, j, k)]; }
+  __device__ __forceinline__ float w(int i, int j, int k) const { return weight[idx(i, j, k)]; }
+  __device__ __forceinline__ float c(int i, int j, int k, int ch) const { return color[idx(i, j, k) * 3 + ch]; }
+  __device__ __forceinline__ DenseVox bind(size_t v, int& i, int& j, int& k) const {
+    i = (int)(v % nx);
+    j = (int)((v / nx) % ny);
+    k = (int)(v / ((size_t)nx * ny));
+    return *this;
+  }
+  __device__ __forceinline__ void pos(int i, int j, int k, int* p) const { p[0] = i; p[1] = j; p[2] = k; }
+  // record key of the voxel at offset (dx,dy,dz) in {0,1}^3 from record key `key`, and the records to search for it:
+  // keys are distinct and ascending, so it lies within (owner - key) places after r
+  __device__ __forceinline__ int owner(int key, int dx, int dy, int dz, int r, int n, int& lo, int& hi) const {
+    const int own = key + dx + dy * nx + dz * nx * ny;     // grids are limited to < 2^31 voxels
+    lo = r; hi = min(n - 1, r + (own - key));
+    return own;
+  }
+};
+
+// block volume: pool [B,16,16,16] (x fastest); record key = pool index * 4096 + local voxel.  A bound accessor holds the
+// pool block's row of the neighbour table [B,27] (-1 = unallocated; offset (a,b,c) in {-1,0,1}^3 at (a+1)+3(b+1)+9(c+1))
+// and reads any voxel at accessor coordinates in [-16, 32) through it.
+struct BlockVox {
+  const float* tsdf;
+  const float* weight;
+  const float* color;
+  const int* nbr;           // [B,27]
+  const int* coords;        // [B,3] block coordinates
+  const int* row;           // bound: nbr + 27 * pool index
+  int bc[3];                // bound: block coordinate
+  __device__ __forceinline__ long long idx(int i, int j, int k) const {
+    const int q = row[((i >> 4) + 1) + 3 * ((j >> 4) + 1) + 9 * ((k >> 4) + 1)];
+    return q < 0 ? -1 : ((long long)q << 12) + ((k & 15) << 8) + ((j & 15) << 4) + (i & 15);
+  }
+  __device__ __forceinline__ bool inside(int, int, int) const { return true; }
+  __device__ __forceinline__ float t(int i, int j, int k) const { const long long v = idx(i, j, k); return v < 0 ? 0.f : tsdf[v]; }
+  __device__ __forceinline__ float w(int i, int j, int k) const { const long long v = idx(i, j, k); return v < 0 ? 0.f : weight[v]; }
+  __device__ __forceinline__ float c(int i, int j, int k, int ch) const {
+    const long long v = idx(i, j, k);
+    return v < 0 ? 0.f : color[v * 3 + ch];
+  }
+  __device__ __forceinline__ BlockVox bind(size_t v, int& i, int& j, int& k) const {
+    const int p = (int)(v >> 12), l = (int)(v & 4095);
+    i = l & 15; j = (l >> 4) & 15; k = l >> 8;
+    BlockVox b = *this;
+    b.row = nbr + 27 * (size_t)p;
+    for (int q = 0; q < 3; q++) b.bc[q] = coords[3 * (size_t)p + q];
+    return b;
+  }
+  __device__ __forceinline__ void pos(int i, int j, int k, int* p) const { p[0] = 16 * bc[0] + i; p[1] = 16 * bc[1] + j; p[2] = 16 * bc[2] + k; }
+  // the owner may sit in a block of lower pool index: search below r or above it
+  __device__ __forceinline__ int owner(int key, int dx, int dy, int dz, int r, int n, int& lo, int& hi) const {
+    const int l = key & 4095, i = (l & 15) + dx, j = ((l >> 4) & 15) + dy, k = (l >> 8) + dz;
+    const int q = nbr[27 * (size_t)(key >> 12) + ((i >> 4) + 1) + 3 * ((j >> 4) + 1) + 9 * ((k >> 4) + 1)];
+    const int own = q < 0 ? -1 : (q << 12) + ((k & 15) << 8) + ((j & 15) << 4) + (i & 15);
+    if (own >= key) { lo = r; hi = min(n - 1, r + (own - key)); } else { lo = 0; hi = r; }
+    return own;
+  }
 };
 
 __device__ __forceinline__ int tri_count(int cs) {
@@ -123,31 +190,30 @@ __device__ __forceinline__ int tri_count(int cs) {
 }
 
 // voxel (i,j,k) -> vertex mask (bits 0-2: its +x, +y, +z edges carry a vertex) | case << 3 | cube valid << 11
-__device__ int mesh_classify(const MeshVolume& g, int i, int j, int k) {
-  const size_t sy = (size_t)g.nx, sz = (size_t)g.nx * g.ny;
-  const size_t v = (size_t)k * sz + (size_t)j * sy + i;
-  const bool hx = i + 1 < g.nx, hy = j + 1 < g.ny, hz = k + 1 < g.nz;
-  const bool n0 = g.tsdf[v] < 0.f;
-  const bool cx = hx && ((g.tsdf[v + 1] < 0.f) != n0);
-  const bool cy = hy && ((g.tsdf[v + sy] < 0.f) != n0);
-  const bool cz = hz && ((g.tsdf[v + sz] < 0.f) != n0);
+template <class V>
+__device__ int mesh_classify(const V& g, int i, int j, int k, float min_weight) {
+  const bool hx = g.inside(i + 1, j, k), hy = g.inside(i, j + 1, k), hz = g.inside(i, j, k + 1);
+  const bool n0 = g.t(i, j, k) < 0.f;
+  const bool cx = hx && ((g.t(i + 1, j, k) < 0.f) != n0);
+  const bool cy = hy && ((g.t(i, j + 1, k) < 0.f) != n0);
+  const bool cz = hz && ((g.t(i, j, k + 1) < 0.f) != n0);
   int cs = 0;
   if (hx && hy && hz) {
 #pragma unroll
     for (int n = 0; n < 8; n++) {
       const int dx = (n == 1 || n == 2 || n == 5 || n == 6), dy = (n == 2 || n == 3 || n == 6 || n == 7), dz = n >= 4;
-      cs |= (g.tsdf[v + dx + dy * sy + dz * sz] < 0.f) << n;
+      cs |= (g.t(i + dx, j + dy, k + dz) < 0.f) << n;
     }
   }
   if (!(cx || cy || cz) && (cs == 0 || cs == 255)) return 0;
-  // weight test over the 3x3x3 neighbourhood: bit (a+1) + 3(b+1) + 9(c+1) for offset (a,b,c); outside the grid = fails
+  // weight test over the 3x3x3 neighbourhood: bit (a+1) + 3(b+1) + 9(c+1) for offset (a,b,c); a missing voxel fails
   unsigned ok = 0;
   for (int c = -1; c <= 1; c++)
     for (int b = -1; b <= 1; b++)
       for (int a = -1; a <= 1; a++) {
         const int ii = i + a, jj = j + b, kk = k + c;
-        if (ii < 0 || jj < 0 || kk < 0 || ii >= g.nx || jj >= g.ny || kk >= g.nz) continue;
-        if (g.weight[(size_t)kk * sz + (size_t)jj * sy + ii] > g.min_weight) ok |= 1u << ((a + 1) + 3 * (b + 1) + 9 * (c + 1));
+        if (!g.inside(ii, jj, kk)) continue;
+        if (g.w(ii, jj, kk) > min_weight) ok |= 1u << ((a + 1) + 3 * (b + 1) + 9 * (c + 1));
       }
   // cube at offset (a,b,c) in {-1,0}^3 is valid when its 8 corner bits are set: mask 0x361B shifted by (a+1)+3(b+1)+9(c+1)
   auto cube = [ok](int s) { return ((ok >> s) & 0x361Bu) == 0x361Bu; };
@@ -163,12 +229,6 @@ __device__ __forceinline__ void mesh_counts(int bits, int& nv, int& nt, int& na)
   nv = __popc(bits & 7);
   nt = (bits >> 11) & 1 ? tri_count((bits >> 3) & 255) : 0;
   na = (nv | nt) != 0;
-}
-
-__device__ __forceinline__ void voxel_ijk(const MeshVolume& g, size_t v, int& i, int& j, int& k) {
-  i = (int)(v % g.nx);
-  j = (int)((v / g.nx) % g.ny);
-  k = (int)(v / ((size_t)g.nx * g.ny));
 }
 
 // exclusive scan of (x, y, z) over the block; totals returned in tx, ty, tz.  blockDim.x = NT, a multiple of 32
@@ -203,13 +263,14 @@ __device__ __forceinline__ void block_scan3(int& x, int& y, int& z, int& tx, int
 }
 
 // pass 1: per-block counts of vertices, triangles, active voxels -> scratch[4 + 3 * block + {0,1,2}]
-__global__ void __launch_bounds__(kMeshBlock, 4) tsdf_mesh_classify_kernel(MeshVolume g, size_t nvox, int* scratch) {
+template <class V>
+__global__ void __launch_bounds__(kMeshBlock, 4) tsdf_mesh_classify_kernel(V g, size_t nvox, float min_weight, int* scratch) {
   const size_t v = (size_t)blockIdx.x * kMeshBlock + threadIdx.x;
   int nv = 0, nt = 0, na = 0;
   if (v < nvox) {
     int i, j, k;
-    voxel_ijk(g, v, i, j, k);
-    mesh_counts(mesh_classify(g, i, j, k), nv, nt, na);
+    const V b = g.bind(v, i, j, k);
+    mesh_counts(mesh_classify(b, i, j, k, min_weight), nv, nt, na);
   }
   int tv, tt, ta;
   block_scan3<kMeshBlock>(nv, nt, na, tv, tt, ta);
@@ -246,7 +307,8 @@ __global__ void __launch_bounds__(kScanThreads) tsdf_mesh_scan_kernel(int* scrat
 
 struct MeshOut {
   float ox, oy, oz, voxel;
-  int4* active;             // [A] (voxel index, vertex base, triangle base, classify bits)
+  float min_weight;
+  int4* active;             // [A] (record key, vertex base, triangle base, classify bits)
   int n_active;
   float* vertices;          // [V,3]
   float* colors;            // [V,3] in [0,1]
@@ -254,53 +316,51 @@ struct MeshOut {
   int* triangles;           // [T,3]
 };
 
-// TSDF gradient component along one axis at voxel (i,j,k): central difference, one-sided at the border
-__device__ __forceinline__ float tsdf_grad(const MeshVolume& g, size_t v, int idx, int n, size_t stride) {
-  if (n < 2) return 0.f;
-  if (idx == 0) return __fsub_rn(g.tsdf[v + stride], g.tsdf[v]);
-  if (idx == n - 1) return __fsub_rn(g.tsdf[v], g.tsdf[v - stride]);
-  return __fmul_rn(__fsub_rn(g.tsdf[v + stride], g.tsdf[v - stride]), 0.5f);
+// TSDF gradient component along `axis` at voxel p: central difference, one-sided where a neighbour is missing
+template <class V>
+__device__ __forceinline__ float tsdf_grad(const V& g, const int* p, int axis) {
+  int lo[3] = {p[0], p[1], p[2]}, hi[3] = {p[0], p[1], p[2]};
+  lo[axis] -= 1; hi[axis] += 1;
+  const bool has_lo = g.inside(lo[0], lo[1], lo[2]), has_hi = g.inside(hi[0], hi[1], hi[2]);
+  if (!has_lo && !has_hi) return 0.f;
+  if (!has_lo) return __fsub_rn(g.t(hi[0], hi[1], hi[2]), g.t(p[0], p[1], p[2]));
+  if (!has_hi) return __fsub_rn(g.t(p[0], p[1], p[2]), g.t(lo[0], lo[1], lo[2]));
+  return __fmul_rn(__fsub_rn(g.t(hi[0], hi[1], hi[2]), g.t(lo[0], lo[1], lo[2])), 0.5f);
 }
 
-__device__ __forceinline__ float lerp_rn(float a, float b, float t) { return __fadd_rn(a, __fmul_rn(t, __fsub_rn(b, a))); }
-
-__device__ void emit_vertex(const MeshVolume& g, const MeshOut& o, int i, int j, int k, size_t v, int axis, int id) {
-  const size_t sy = (size_t)g.nx, sz = (size_t)g.nx * g.ny;
-  const size_t s = axis == 0 ? 1 : axis == 1 ? sy : sz;
-  const float f0 = g.tsdf[v], f1 = g.tsdf[v + s];
+template <class V>
+__device__ void emit_vertex(const V& g, const MeshOut& o, int i, int j, int k, int axis, int id) {
+  int p0[3] = {i, j, k}, p1[3] = {i, j, k};
+  p1[axis] += 1;
+  const float f0 = g.t(i, j, k), f1 = g.t(p1[0], p1[1], p1[2]);
   const float t = __fdiv_rn(f0, __fsub_rn(f0, f1));
-  float idx[3] = {(float)i, (float)j, (float)k};
+  int li[3];
+  g.pos(i, j, k, li);
+  float idx[3] = {(float)li[0], (float)li[1], (float)li[2]};
   idx[axis] = __fadd_rn(idx[axis], t);
   const float org[3] = {o.ox, o.oy, o.oz};
   const size_t w = (size_t)id * 3;
 #pragma unroll
   for (int a = 0; a < 3; a++) o.vertices[w + a] = __fadd_rn(org[a], __fmul_rn(o.voxel, idx[a]));
 #pragma unroll
-  for (int c = 0; c < 3; c++) o.colors[w + c] = __fdiv_rn(lerp_rn(g.color[v * 3 + c], g.color[(v + s) * 3 + c], t), 255.f);
-  int p0[3] = {i, j, k}, p1[3] = {i, j, k};
-  p1[axis] += 1;
-  const int dims[3] = {g.nx, g.ny, g.nz};
-  const size_t str[3] = {1, sy, sz};
+  for (int c = 0; c < 3; c++) o.colors[w + c] = __fdiv_rn(lerp_rn(g.c(i, j, k, c), g.c(p1[0], p1[1], p1[2], c), t), 255.f);
   float n[3];
 #pragma unroll
-  for (int a = 0; a < 3; a++) {
-    const float g0 = tsdf_grad(g, v, p0[a], dims[a], str[a]);
-    const float g1 = tsdf_grad(g, v + s, p1[a], dims[a], str[a]);
-    n[a] = lerp_rn(g0, g1, t);
-  }
+  for (int a = 0; a < 3; a++) n[a] = lerp_rn(tsdf_grad(g, p0, a), tsdf_grad(g, p1, a), t);
   const float len = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(n[0], n[0]), __fmul_rn(n[1], n[1])), __fmul_rn(n[2], n[2])));
 #pragma unroll
   for (int a = 0; a < 3; a++) o.normals[w + a] = len > 0.f ? __fdiv_rn(n[a], len) : 0.f;
 }
 
-// pass 3: active-voxel records in ascending voxel order and the vertices
-__global__ void __launch_bounds__(kMeshBlock) tsdf_mesh_compact_kernel(MeshVolume g, size_t nvox, const int* scratch,
-                                                                       MeshOut o) {
+// pass 3: active-voxel records in ascending key order and the vertices
+template <class V>
+__global__ void __launch_bounds__(kMeshBlock) tsdf_mesh_compact_kernel(V g, size_t nvox, const int* scratch, MeshOut o) {
   const size_t v = (size_t)blockIdx.x * kMeshBlock + threadIdx.x;
   int bits = 0, i = 0, j = 0, k = 0;
+  V b = g;
   if (v < nvox) {
-    voxel_ijk(g, v, i, j, k);
-    bits = mesh_classify(g, i, j, k);
+    b = g.bind(v, i, j, k);
+    bits = mesh_classify(b, i, j, k, o.min_weight);
   }
   int nv, nt, na;
   mesh_counts(bits, nv, nt, na);
@@ -308,29 +368,29 @@ __global__ void __launch_bounds__(kMeshBlock) tsdf_mesh_compact_kernel(MeshVolum
   int tv, tt, ta;
   block_scan3<kMeshBlock>(nv, nt, na, tv, tt, ta);
   if (!is_active) return;
-  const int* b = scratch + 4 + 3 * (size_t)blockIdx.x;
-  const int vbase = b[0] + nv, tbase = b[1] + nt, r = b[2] + na;
+  const int* c = scratch + 4 + 3 * (size_t)blockIdx.x;
+  const int vbase = c[0] + nv, tbase = c[1] + nt, r = c[2] + na;
   o.active[r] = make_int4((int)v, vbase, tbase, bits);
   int id = vbase;
   for (int a = 0; a < 3; a++)
-    if ((bits >> a) & 1) emit_vertex(g, o, i, j, k, v, a, id++);
+    if ((bits >> a) & 1) emit_vertex(b, o, i, j, k, a, id++);
 }
 
-// pass 4: triangles of every active voxel whose cube is valid
-__global__ void __launch_bounds__(kMeshBlock) tsdf_mesh_triangles_kernel(MeshVolume g, MeshOut o) {
+// pass 4: triangles of every active voxel whose cube is valid; each edge resolved to its owner's record by binary search
+template <class V>
+__global__ void __launch_bounds__(kMeshBlock) tsdf_mesh_triangles_kernel(V g, MeshOut o) {
   const int r = blockIdx.x * kMeshBlock + threadIdx.x;
   if (r >= o.n_active) return;
   const int4 rec = o.active[r];
   if (!((rec.w >> 11) & 1)) return;
   const int cs = (rec.w >> 3) & 255;
   const int nt = tri_count(cs);
-  const int sy = g.nx, sz = g.nx * g.ny;                 // grids are limited to < 2^31 voxels
   for (int s = 0; s < nt; s++)
     for (int q = 0; q < 3; q++) {
       const int eo = c_edge_owner[c_tri[cs][3 * s + q]];
-      const int owner = rec.x + (eo & 1) + ((eo >> 1) & 1) * sy + ((eo >> 2) & 1) * sz, axis = eo >> 3;
-      // records are sorted by distinct voxel index, so the owner's record lies within owner - voxel places after r
-      int lo = r, hi = min(o.n_active - 1, r + (owner - rec.x));
+      const int axis = eo >> 3;
+      int lo, hi;
+      const int owner = g.owner(rec.x, eo & 1, (eo >> 1) & 1, (eo >> 2) & 1, r, o.n_active, lo, hi);
       while (lo < hi) {
         const int mid = (lo + hi) >> 1;
         if (o.active[mid].x < owner) lo = mid + 1; else hi = mid;
@@ -341,134 +401,53 @@ __global__ void __launch_bounds__(kMeshBlock) tsdf_mesh_triangles_kernel(MeshVol
 }
 
 // ---------------------------------------------------------------------------------------------------------------- ray cast
-struct RayArgs {
-  MeshVolume g;
-  float ox, oy, oz, voxel;
-  const float* pose;        // [n,7] cam_T_world (t, q_xyzw), DEVICE
-  int H, W;
-  float fx, fy, cx, cy, min_depth, max_depth, trunc;
-  float* depth;             // [n,H,W]
-  float* color;             // [n,H,W,3]
-  float* weight;            // [n,H,W]
-  float* normal;            // [n,H,W,3] or NULL
-};
-
-struct Cell {
-  size_t v;                 // linear index of the cell's corner (0,0,0)
-  float fx, fy, fz;         // fractions within the cell
-};
-
-__device__ __forceinline__ float tri_lerp(const float* a, size_t sy, size_t sz, size_t v, int ch, int nch, const Cell& c) {
-  auto at = [&](int dx, int dy, int dz) { return a[(v + dx + dy * sy + dz * sz) * nch + ch]; };
-  const float c0 = lerp_rn(lerp_rn(at(0, 0, 0), at(1, 0, 0), c.fx), lerp_rn(at(0, 1, 0), at(1, 1, 0), c.fx), c.fy);
-  const float c1 = lerp_rn(lerp_rn(at(0, 0, 1), at(1, 0, 1), c.fx), lerp_rn(at(0, 1, 1), at(1, 1, 1), c.fx), c.fy);
-  return lerp_rn(c0, c1, c.fz);
-}
-
-__global__ void __launch_bounds__(128) tsdf_raycast_kernel(RayArgs a) {
-  __shared__ double sR[9];
-  __shared__ float sgo[3];
-  const int view = blockIdx.y;
-  if (threadIdx.x == 0) {
-    const float* p = a.pose + 7 * (size_t)view;
-    const double qx = p[3], qy = p[4], qz = p[5], qw = p[6];
-    const double R[9] = {1 - 2 * (qy * qy + qz * qz), 2 * (qx * qy - qz * qw), 2 * (qx * qz + qy * qw),
-                         2 * (qx * qy + qz * qw), 1 - 2 * (qx * qx + qz * qz), 2 * (qy * qz - qx * qw),
-                         2 * (qx * qz - qy * qw), 2 * (qy * qz + qx * qw), 1 - 2 * (qx * qx + qy * qy)};
-    for (int i = 0; i < 9; i++) sR[i] = (double)(float)R[i];       // the fp32 rotation of the pose, as tsdf.cu
-    const double t0 = p[0], t1 = p[1], t2 = p[2];
-    const float org[3] = {a.ox, a.oy, a.oz};
-    for (int c = 0; c < 3; c++) {
-      // camera centre -R^T t, then grid coordinates (world - origin) / voxel
-      const float cw = (float)-__dadd_rn(__dadd_rn(__dmul_rn((double)(float)R[c], t0), __dmul_rn((double)(float)R[3 + c], t1)),
-                                         __dmul_rn((double)(float)R[6 + c], t2));
-      sgo[c] = __fdiv_rn(__fsub_rn(cw, org[c]), a.voxel);
-    }
-  }
-  __syncthreads();
-  const int pix = blockIdx.x * blockDim.x + threadIdx.x;
-  if (pix >= a.H * a.W) return;
-  const int u = pix % a.W, v = pix / a.W;
-  const float dxc = __fdiv_rn(__fsub_rn((float)u, a.cx), a.fx), dyc = __fdiv_rn(__fsub_rn((float)v, a.cy), a.fy);
-  float gd[3];
-#pragma unroll
-  for (int c = 0; c < 3; c++)
-    gd[c] = __fdiv_rn((float)__dadd_rn(__dadd_rn(__dmul_rn(sR[c], (double)dxc), __dmul_rn(sR[3 + c], (double)dyc)), sR[6 + c]),
-                      a.voxel);
-  const float len = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(dxc, dxc), __fmul_rn(dyc, dyc)), 1.f));
-  const MeshVolume& g = a.g;
-  const int dims[3] = {g.nx, g.ny, g.nz};
-  const size_t sy = (size_t)g.nx, sz = (size_t)g.nx * g.ny;
-
-  // grid cell of depth z; false outside the grid
-  auto locate = [&](float z, Cell& c, bool clamp) {
-    float fr[3];
+// dense grid: a sample outside the grid is unobserved; the hit's cell is clamped into the grid
+struct DenseRay {
+  DenseVox g;
+  float min_weight;
+  __device__ __forceinline__ bool locate(const float* gq, size_t& v, float* fr, bool clamp) const {
+    const int dims[3] = {g.nx, g.ny, g.nz};
     int ix[3];
     bool inb = true;
 #pragma unroll
     for (int q = 0; q < 3; q++) {
-      const float gq = __fadd_rn(sgo[q], __fmul_rn(z, gd[q]));
-      float fl = floorf(gq);
+      float fl = floorf(gq[q]);
       if (clamp) fl = fminf(fmaxf(fl, 0.f), (float)(dims[q] - 2));
       inb = inb && fl >= 0.f && fl <= (float)(dims[q] - 2);
       ix[q] = inb ? (int)fl : 0;
-      fr[q] = __fsub_rn(gq, fl);
+      fr[q] = __fsub_rn(gq[q], fl);
     }
-    c.v = (size_t)ix[2] * sz + (size_t)ix[1] * sy + ix[0];
-    c.fx = fr[0]; c.fy = fr[1]; c.fz = fr[2];
+    v = g.idx(ix[0], ix[1], ix[2]);
     return inb;
-  };
-  auto observed = [&](size_t v0) {
-    bool ok = true;
+  }
+  __device__ __forceinline__ size_t corner(size_t v, int n) const {
+    return v + (n & 1) + ((n >> 1) & 1) * (size_t)g.nx + (n >> 2) * (size_t)g.nx * g.ny;
+  }
+  __device__ __forceinline__ bool sample(const float* gq, float& f) const {
+    size_t v;
+    float fr[3];
+    if (!locate(gq, v, fr, false)) return false;
+    for (int n = 0; n < 8; n++)
+      if (!(g.weight[corner(v, n)] > min_weight)) return false;
+    float t[8];
 #pragma unroll
-    for (int n = 0; n < 8; n++) ok = ok && g.weight[v0 + (n & 1) + ((n >> 1) & 1) * sy + (n >> 2) * sz] > g.min_weight;
-    return ok;
-  };
-
-  const int max_steps = (int)ceilf(__fdiv_rn(__fmul_rn(__fsub_rn(a.max_depth, a.min_depth), len), a.voxel)) + 2;
-  float z = a.min_depth, z_prev = 0.f, f_prev = 0.f, z_hit = 0.f;
-  bool have_prev = false, hit = false;
-  for (int s = 0; s < max_steps && z <= a.max_depth; s++) {
-    Cell c;
-    const bool obs = locate(z, c, false) && observed(c.v);
-    const float f = tri_lerp(g.tsdf, sy, sz, c.v, 0, 1, c);
-    if (obs && have_prev && f_prev > 0.f && f <= 0.f) {
-      z_hit = __fadd_rn(z_prev, __fdiv_rn(__fmul_rn(__fsub_rn(z, z_prev), f_prev), __fsub_rn(f_prev, f)));
-      hit = true;
-      break;
+    for (int n = 0; n < 8; n++) t[n] = g.tsdf[corner(v, n)];
+    f = trilerp8(t, fr[0], fr[1], fr[2]);
+    return true;
+  }
+  __device__ __forceinline__ void hit(const float* gq, RayCell& c) const {
+    size_t v;
+    float fr[3];
+    locate(gq, v, fr, true);
+    c.fx = fr[0]; c.fy = fr[1]; c.fz = fr[2];
+#pragma unroll
+    for (int n = 0; n < 8; n++) {
+      const size_t q = corner(v, n);
+      c.t[n] = g.tsdf[q]; c.w[n] = g.weight[q];
+      for (int ch = 0; ch < 3; ch++) c.c[ch][n] = g.color[q * 3 + ch];
     }
-    const float step = obs && f > 0.f ? fmaxf(__fmul_rn(f, a.trunc), a.voxel) : a.voxel;
-    have_prev = obs; f_prev = f; z_prev = z;
-    z = __fadd_rn(z, __fdiv_rn(step, len));
   }
-
-  const size_t o = (size_t)view * a.H * a.W + pix;
-  if (!hit) {
-    a.depth[o] = 0.f; a.weight[o] = 0.f;
-    for (int c = 0; c < 3; c++) a.color[3 * o + c] = 0.f;
-    if (a.normal) for (int c = 0; c < 3; c++) a.normal[3 * o + c] = 0.f;
-    return;
-  }
-  Cell c;
-  locate(z_hit, c, true);
-  a.depth[o] = z_hit;
-  a.weight[o] = tri_lerp(g.weight, sy, sz, c.v, 0, 1, c);
-  for (int ch = 0; ch < 3; ch++) a.color[3 * o + ch] = __fdiv_rn(tri_lerp(g.color, sy, sz, c.v, ch, 3, c), 255.f);
-  if (a.normal) {
-    auto T = [&](int dx, int dy, int dz) { return g.tsdf[c.v + dx + dy * sy + dz * sz]; };
-    auto d = [](float p, float q) { return __fsub_rn(p, q); };
-    const float gx = lerp_rn(lerp_rn(d(T(1, 0, 0), T(0, 0, 0)), d(T(1, 1, 0), T(0, 1, 0)), c.fy),
-                             lerp_rn(d(T(1, 0, 1), T(0, 0, 1)), d(T(1, 1, 1), T(0, 1, 1)), c.fy), c.fz);
-    const float gy = lerp_rn(lerp_rn(d(T(0, 1, 0), T(0, 0, 0)), d(T(1, 1, 0), T(1, 0, 0)), c.fx),
-                             lerp_rn(d(T(0, 1, 1), T(0, 0, 1)), d(T(1, 1, 1), T(1, 0, 1)), c.fx), c.fz);
-    const float gz = lerp_rn(lerp_rn(d(T(0, 0, 1), T(0, 0, 0)), d(T(1, 0, 1), T(1, 0, 0)), c.fx),
-                             lerp_rn(d(T(0, 1, 1), T(0, 1, 0)), d(T(1, 1, 1), T(1, 1, 0)), c.fx), c.fy);
-    const float gl = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(gx, gx), __fmul_rn(gy, gy)), __fmul_rn(gz, gz)));
-    a.normal[3 * o + 0] = gl > 0.f ? __fdiv_rn(gx, gl) : 0.f;
-    a.normal[3 * o + 1] = gl > 0.f ? __fdiv_rn(gy, gl) : 0.f;
-    a.normal[3 * o + 2] = gl > 0.f ? __fdiv_rn(gz, gl) : 0.f;
-  }
-}
+};
 
 // grids whose worst-case vertex (3 per voxel) and triangle (5 per cube) counts fit int32
 static bool mesh_grid_ok(int nx, int ny, int nz) {
@@ -476,6 +455,30 @@ static bool mesh_grid_ok(int nx, int ny, int nz) {
   const long long n = (long long)nx * ny * nz;
   const long long cubes = (long long)(nx - 1) * (ny - 1) * (nz - 1);
   return 3 * n <= INT_MAX && 5 * cubes <= INT_MAX;
+}
+
+// block pools whose worst-case vertex and triangle counts (3 and 5 per voxel) fit int32
+static bool mesh_blocks_ok(int n_blocks) { return n_blocks >= 0 && 5LL * 4096 * n_blocks <= INT_MAX; }
+
+template <class V>
+static int mesh_count(const V& g, size_t n, float min_weight, int* scratch, void* stream) {
+  const int nblocks = (int)((n + kMeshBlock - 1) / kMeshBlock);
+  tsdf_mesh_classify_kernel<<<nblocks, kMeshBlock, 0, (cudaStream_t)stream>>>(g, n, min_weight, scratch);
+  NSLAM_CHECK_LAUNCH();
+  tsdf_mesh_scan_kernel<<<1, kScanThreads, 0, (cudaStream_t)stream>>>(scratch, nblocks);
+  NSLAM_CHECK_LAUNCH();
+  return 0;
+}
+
+template <class V>
+static int mesh_emit(const V& g, size_t n, const int* scratch, const MeshOut& o, void* stream) {
+  if (o.n_active == 0) return 0;
+  const int nblocks = (int)((n + kMeshBlock - 1) / kMeshBlock);
+  tsdf_mesh_compact_kernel<<<nblocks, kMeshBlock, 0, (cudaStream_t)stream>>>(g, n, scratch, o);
+  NSLAM_CHECK_LAUNCH();
+  tsdf_mesh_triangles_kernel<<<(o.n_active + kMeshBlock - 1) / kMeshBlock, kMeshBlock, 0, (cudaStream_t)stream>>>(g, o);
+  NSLAM_CHECK_LAUNCH();
+  return 0;
 }
 
 }  // namespace nslam
@@ -498,14 +501,7 @@ int nslam_tsdf_mesh_count(const float* tsdf, const float* weight, int nx, int ny
                           void* stream) {
   using namespace nslam;
   if (!mesh_grid_ok(nx, ny, nz)) return (int)cudaErrorInvalidValue;
-  const size_t n = (size_t)nx * ny * nz;
-  const int nblocks = (int)((n + kMeshBlock - 1) / kMeshBlock);
-  MeshVolume g{tsdf, weight, nullptr, nx, ny, nz, min_weight};
-  tsdf_mesh_classify_kernel<<<nblocks, kMeshBlock, 0, (cudaStream_t)stream>>>(g, n, scratch);
-  NSLAM_CHECK_LAUNCH();
-  tsdf_mesh_scan_kernel<<<1, kScanThreads, 0, (cudaStream_t)stream>>>(scratch, nblocks);
-  NSLAM_CHECK_LAUNCH();
-  return 0;
+  return mesh_count(DenseVox{tsdf, weight, nullptr, nx, ny, nz}, (size_t)nx * ny * nz, min_weight, scratch, stream);
 }
 
 /* Marching cubes, emission passes after nslam_tsdf_mesh_count with the same volume and min_weight: active [n_active,4]
@@ -517,17 +513,9 @@ int nslam_tsdf_mesh_emit(const float* tsdf, const float* weight, const float* co
                          void* stream) {
   using namespace nslam;
   if (!mesh_grid_ok(nx, ny, nz) || n_active < 0) return (int)cudaErrorInvalidValue;
-  if (n_active == 0) return 0;
-  const size_t n = (size_t)nx * ny * nz;
-  const int nblocks = (int)((n + kMeshBlock - 1) / kMeshBlock);
-  MeshVolume g{tsdf, weight, color, nx, ny, nz, min_weight};
-  MeshOut o{origin3_host[0], origin3_host[1], origin3_host[2], voxel_size, (int4*)active, n_active,
+  MeshOut o{origin3_host[0], origin3_host[1], origin3_host[2], voxel_size, min_weight, (int4*)active, n_active,
             vertices, vertex_colors, vertex_normals, triangles};
-  tsdf_mesh_compact_kernel<<<nblocks, kMeshBlock, 0, (cudaStream_t)stream>>>(g, n, scratch, o);
-  NSLAM_CHECK_LAUNCH();
-  tsdf_mesh_triangles_kernel<<<(n_active + kMeshBlock - 1) / kMeshBlock, kMeshBlock, 0, (cudaStream_t)stream>>>(g, o);
-  NSLAM_CHECK_LAUNCH();
-  return 0;
+  return mesh_emit(DenseVox{tsdf, weight, color, nx, ny, nz}, (size_t)nx * ny * nz, scratch, o, stream);
 }
 
 /* Ray cast n views of the volume in one launch: cam_T_world_tq [n,7] (t, q_xyzw) DEVICE; intr4 = fx, fy, cx, cy (HOST);
@@ -541,17 +529,50 @@ int nslam_tsdf_raycast(const float* tsdf, const float* weight, const float* colo
   if (nx < 2 || ny < 2 || nz < 2 || n < 0 || H <= 0 || W <= 0 || n > 65535 || (long long)H * W > INT_MAX)
     return (int)cudaErrorInvalidValue;
   if (n == 0) return 0;
-  RayArgs a{};
-  a.g = MeshVolume{tsdf, weight, color, nx, ny, nz, min_weight};
-  a.ox = origin3_host[0]; a.oy = origin3_host[1]; a.oz = origin3_host[2]; a.voxel = voxel_size;
-  a.pose = cam_T_world_tq; a.H = H; a.W = W;
-  a.fx = intr4_host[0]; a.fy = intr4_host[1]; a.cx = intr4_host[2]; a.cy = intr4_host[3];
-  a.min_depth = min_depth; a.max_depth = max_depth; a.trunc = sdf_trunc;
-  a.depth = depth; a.color = color_out; a.weight = weight_out; a.normal = normal_out;
+  const RayParams a = ray_params(origin3_host, voxel_size, cam_T_world_tq, H, W, intr4_host, min_depth, max_depth,
+                                 sdf_trunc, depth, color_out, weight_out, normal_out);
   dim3 grid((unsigned)(((long long)H * W + 127) / 128), n);
-  tsdf_raycast_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(a);
+  tsdf_raycast_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(a, DenseRay{DenseVox{tsdf, weight, color, nx, ny, nz}, min_weight});
   NSLAM_CHECK_LAUNCH();
   return 0;
+}
+
+/* Marching cubes over a voxel-block volume (csrc/tsdf_blocks.cu): the dense read-out of the volume's dense embedding
+ * (tsdf, weight, colour 0 outside its blocks) at lattice origin 0.  Scratch size (int32 elements): 4 + 48 per block;
+ * cudaErrorInvalidValue when the worst-case vertex or triangle count of n_blocks blocks overflows int32. */
+int nslam_tsdf_blocks_mesh_plan(int n_blocks, long long* scratch_ints) {
+  using namespace nslam;
+  if (!mesh_blocks_ok(n_blocks)) return (int)cudaErrorInvalidValue;
+  *scratch_ints = 4 + 3 * ((4096LL * n_blocks + kMeshBlock - 1) / kMeshBlock);
+  return 0;
+}
+
+/* Counting passes over the pool: tsdf / weight [B,16,16,16], neighbours [B,27] (nslam_tsdf_blocks_neighbours), block
+ * coordinates [B,3] int32 (DEVICE).  min_weight >= 0, so that no voxel outside the blocks is observed. */
+int nslam_tsdf_blocks_mesh_count(const float* tsdf, const float* weight, const int* neighbours, const int* block_coords,
+                                 int n_blocks, float min_weight, int* scratch, void* stream) {
+  using namespace nslam;
+  if (!mesh_blocks_ok(n_blocks) || !(min_weight >= 0.f)) return (int)cudaErrorInvalidValue;
+  if (n_blocks == 0) {
+    cudaMemsetAsync(scratch, 0, 4 * sizeof(int), (cudaStream_t)stream);
+    NSLAM_CHECK_LAUNCH();
+    return 0;
+  }
+  return mesh_count(BlockVox{tsdf, weight, nullptr, neighbours, block_coords, nullptr, {0, 0, 0}}, 4096 * (size_t)n_blocks,
+                    min_weight, scratch, stream);
+}
+
+/* Emission passes after nslam_tsdf_blocks_mesh_count, as nslam_tsdf_mesh_emit.  Vertices are ordered by (pool index,
+ * local voxel, axis), triangles by (pool index, local cube, table order); positions are voxel_size * lattice index. */
+int nslam_tsdf_blocks_mesh_emit(const float* tsdf, const float* weight, const float* color, const int* neighbours,
+                                const int* block_coords, int n_blocks, float voxel_size, float min_weight, const int* scratch,
+                                int n_active, int* active, float* vertices, float* vertex_colors, float* vertex_normals,
+                                int* triangles, void* stream) {
+  using namespace nslam;
+  if (!mesh_blocks_ok(n_blocks) || n_active < 0 || !(min_weight >= 0.f)) return (int)cudaErrorInvalidValue;
+  MeshOut o{0.f, 0.f, 0.f, voxel_size, min_weight, (int4*)active, n_active, vertices, vertex_colors, vertex_normals, triangles};
+  return mesh_emit(BlockVox{tsdf, weight, color, neighbours, block_coords, nullptr, {0, 0, 0}}, 4096 * (size_t)n_blocks,
+                   scratch, o, stream);
 }
 
 }  // extern "C"

@@ -18,13 +18,20 @@ Differences by design: Open3D's hashed VoxelBlockGrid driven from Python (~40 te
 synchronisations per keyframe, :185-302) becomes one kernel launch per keyframe on a DENSE grid (csrc/tsdf.cu) —
 the reference's own extent "6 m / 512 voxels" is 2.7 GB at 20 B per voxel on an 80 GB part; poses, depths, weights and
 masks are consumed where the SLAM packet holds them (device tensors; the reference converts each frame to three Open3D
-images and copies the poses to the host)."""
+images and copies the poses to the host).
+
+`args.tsdf_volume = "blocks"` (default "dense") selects the sparse voxel-block volume of tsdf_blocks.py instead: unbounded,
+16^3 blocks allocated where the depth maps reach (`args.tsdf_block_count` to start with, default 5000, the reference's
+block_count), only the voxels of the blocks a keyframe touches updated, as in the reference — so the two volumes update
+different voxel sets, and the choice is the user's.  Integration, the history rebuild, the reset, both read-outs, the
+GUI packets and `--eval` work on either; `surface_points` is dense-only."""
 import csv
 
 import numpy as np
 import torch
 
 from . import _lib
+from .tsdf_blocks import VoxelBlockVolume
 
 
 class TsdfMesh:
@@ -94,10 +101,21 @@ class TsdfFusion:
         # 5000 x 16^3 voxels of capacity; the default here covers its "6 m room")
         self.grid_resolution = int(getattr(args, "tsdf_resolution", 512))
         self.grid_center = np.asarray(getattr(args, "tsdf_center", (0.0, 0.0, 0.0)), np.float32)
+        self.volume_type = getattr(args, "tsdf_volume", "dense")
+        if self.volume_type not in ("dense", "blocks"):
+            raise ValueError(f"tsdf_volume must be 'dense' or 'blocks', not {self.volume_type!r}")
+        self.block_count = int(getattr(args, "tsdf_block_count", 5000))
+        self.volume = None                               # the VoxelBlockVolume in "blocks" mode
         self.integrated_frames = 0
         self.initialize()
 
     def initialize(self):
+        if self.volume_type == "blocks":
+            if self.volume is None:
+                self.volume = VoxelBlockVolume(self.voxel_size, self.block_count, self.device)
+            else:
+                self.volume.reset(self.voxel_size)       # capacity kept
+            return
         n = self.grid_resolution
         dev = self.device
         self.tsdf = torch.zeros(n, n, n, dtype=torch.float32, device=dev)
@@ -213,8 +231,8 @@ class TsdfFusion:
 
     # ------------------------------------------------------------------ integration (:185-302)
     def build_volume(self, packet, intrinsics, masks=None):
-        """every keyframe of the packet into the volume: one kernel launch each, no host synchronisation"""
-        lib = _lib.load()
+        """every keyframe of the packet into the volume: one kernel launch each and no host synchronisation on the dense
+        grid; activation, insertion and integration with one host read each on the block volume"""
         poses = packet["cam0_poses"].to(self.device, torch.float32).contiguous()
         idepths = packet["cam0_idepths_up"].to(self.device, torch.float32).contiguous()
         covs = packet["cam0_depths_cov_up"]
@@ -223,6 +241,13 @@ class TsdfFusion:
         assert images.dtype == torch.uint8 and images.shape[1] == 3
         n, _, H, W = images.shape
         intr = np.ascontiguousarray(np.asarray(intrinsics, np.float32))
+        if self.volume is not None:
+            for k in range(n):                           # one host read of the block counts per keyframe
+                self.volume.integrate(idepths[k], covs[k] if covs is not None else None, images[k], intr, poses[k],
+                                      self.max_depth, self.sdf_trunc, self.max_weight, self.max_depth_sigma_thresh)
+            self.integrated_frames += n
+            return
+        lib = _lib.load()
         n3 = self.grid_resolution
         with _lib.fixed_stream():
             for k in range(n):
@@ -244,7 +269,9 @@ class TsdfFusion:
     # ------------------------------------------------------------------ read-out
     def surface_points(self, min_weight=0.01, max_points=2_000_000):
         """voxel centres next to a zero crossing of the TSDF along x / y / z with enough weight (a quick look at the
-        surface in plain torch; build_mesh is the full read-out) -> [m,3] world points, [m,3] colours"""
+        surface in plain torch; build_mesh is the full read-out) -> [m,3] world points, [m,3] colours.  Dense grid only."""
+        if self.volume is not None:
+            raise NotImplementedError("surface_points reads the dense grid; use build_mesh with tsdf_volume='blocks'")
         t, w = self.tsdf, self.weight
         ok = w > min_weight
         m = torch.zeros_like(ok)
@@ -259,6 +286,8 @@ class TsdfFusion:
     def build_mesh(self, min_weight_for_mesh):
         """:556-573: marching cubes over the cubes whose 8 corners have weight > min_weight_for_mesh -> TsdfMesh, or None
         when there is no triangle.  One host read of the three counts sizes the outputs."""
+        if self.volume is not None:
+            return self.volume.build_mesh(min_weight_for_mesh)
         lib = _lib.load()
         nz, ny, nx = self.tsdf.shape
         dev = self.tsdf.device
@@ -291,9 +320,7 @@ class TsdfFusion:
         if not packet:
             print("Error: asked to render volume, but packet is None.")
             return None
-        lib = _lib.load()
-        dev = self.tsdf.device
-        nz, ny, nx = self.tsdf.shape
+        dev = torch.device(self.device) if self.volume is not None else self.tsdf.device
         poses = packet["cam0_poses"].to(dev, torch.float32).contiguous()
         images = packet["cam0_images"]
         n, (H, W) = poses.shape[0], images.shape[-2:]
@@ -306,11 +333,16 @@ class TsdfFusion:
         with _lib.fixed_stream():
             for s in range(0, n, chunk):
                 m = min(chunk, n - s)
-                _lib.check(lib.nslam_tsdf_raycast(
-                    _lib.ptr(self.tsdf), _lib.ptr(self.weight), _lib.ptr(self.color), nx, ny, nz, self.origin.ctypes.data,
-                    float(self.voxel_size), _lib.ptr(poses[s:s + m]), m, H, W, intr.ctypes.data, float(self.min_depth),
-                    float(self.max_depth), float(self.sdf_trunc), float(min_weight_for_render), _lib.ptr(depth[s:s + m]),
-                    _lib.ptr(color[s:s + m]), _lib.ptr(weight), None, _lib.stream_ptr()), "tsdf_raycast")
+                if self.volume is not None:
+                    depth[s:s + m], color[s:s + m] = self.volume.raycast(
+                        poses[s:s + m], H, W, intr, self.min_depth, self.max_depth, self.sdf_trunc, min_weight_for_render)[:2]
+                else:
+                    nz, ny, nx = self.tsdf.shape
+                    _lib.check(_lib.load().nslam_tsdf_raycast(
+                        _lib.ptr(self.tsdf), _lib.ptr(self.weight), _lib.ptr(self.color), nx, ny, nz, self.origin.ctypes.data,
+                        float(self.voxel_size), _lib.ptr(poses[s:s + m]), m, H, W, intr.ctypes.data, float(self.min_depth),
+                        float(self.max_depth), float(self.sdf_trunc), float(min_weight_for_render), _lib.ptr(depth[s:s + m]),
+                        _lib.ptr(color[s:s + m]), _lib.ptr(weight), None, _lib.stream_ptr()), "tsdf_raycast")
                 if evaluate:
                     for i in range(s, s + m):
                         total_psnr += color_psnr(color[i], images[i])
