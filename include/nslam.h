@@ -134,7 +134,8 @@ int nslam_tsdf_integrate(float* tsdf, float* weight, float* color, int nx, int n
  * triangle count overflows int32); _count -> scratch[0..2] = vertices, triangles, active voxels (DEVICE); _emit with the
  * same volume and min_weight -> active [A,4] int32 scratch, vertices / vertex_colors ([0,1]) / vertex_normals [V,3] fp32,
  * triangles [T,3] int32 in a fixed order (vertices by owning voxel then axis, triangles by cube then table order).
- * A cube is meshed when its 8 corners have weight > min_weight.  origin3 (HOST) as above. */
+ * A cube is meshed when its 8 corners have weight > min_weight.  origin3 (HOST) as above.  color may be NULL (a volume
+ * without colours, such as the NeRF mesh lattice): vertex colours are then 0. */
 int nslam_tsdf_mesh_plan(int nx, int ny, int nz, long long* scratch_ints);
 int nslam_tsdf_mesh_count(const float* tsdf, const float* weight, int nx, int ny, int nz, float min_weight, int* scratch,
                           void* stream);

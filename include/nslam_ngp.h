@@ -115,6 +115,17 @@ int nslam_ngp_train_step_tc(const nslam_ngp_model* m, const nslam_ngp_images* im
 int nslam_ngp_loss_backward_tc(const nslam_ngp_model* m, const nslam_ngp_batch* b, const void* packed, int n_rays,
                                int n_samples, float lambda_depth, float bg_r, float bg_g, float bg_b,
                                float loss_scale, int num_sms, void* stream);
+/* Mesh read-out of the NeRF (Testbed.compute_marching_cubes_mesh; csrc/ngp_tc.cu).  _lattice: density of every point
+ * (i,j,k) of the [nz,ny,nx] lattice at lo3_host (HOST) + h (i,j,k) in the training cameras' world frame, through the
+ * tensor-core density head (encode -> layers 1-2) -> field = thresh - sigma (negative inside), weight = 1 where the
+ * point's occupancy cell (cascade of the finest box holding it) was seen by a training camera, else 0 [nz,ny,nx] fp32
+ * (DEVICE); marching cubes of nslam_tsdf_mesh_* with min_weight 0 and color NULL follow.  _colors: colors [n,3] = network
+ * radiance at the vertices [n,3] seen along -normals [n,3] (+z where the normal is 0), through the tensor-core forward;
+ * srgb != 0: encoded with the inverse of the ingest's sRGB -> linear curve.  `packed` as for forward_tc. */
+int nslam_ngp_mesh_lattice(const nslam_ngp_model* m, const void* packed, const float* lo3_host, float h, int nx, int ny,
+                           int nz, float thresh, float* field, float* weight, int num_sms, void* stream);
+int nslam_ngp_mesh_colors(const nslam_ngp_model* m, const void* packed, const float* vertices, const float* normals, int n,
+                          int srgb, float* colors, int num_sms, void* stream);
 /* the non-network phases of a step (shared by both variants) */
 int nslam_ngp_sample_phase(const nslam_ngp_model* m, const nslam_ngp_images* im, const nslam_ngp_batch* b,
                            int n_rays, unsigned seed, void* stream);

@@ -135,6 +135,8 @@ _SIGNATURES = {
     "nslam_ngp_loss_backward_tc": [_P, _P, _P, c_int, c_int, c_float, c_float, c_float, c_float, c_float, c_int, _P],
     "nslam_ngp_sample_phase": [_P, _P, _P, c_int, ctypes.c_uint, _P],
     "nslam_ngp_loss_phase": [_P, c_int, c_float, c_float, c_float, c_float, _P],
+    "nslam_ngp_mesh_lattice": [_P, _P, _P, c_float, c_int, c_int, c_int, c_float, _P, _P, c_int, _P],
+    "nslam_ngp_mesh_colors": [_P, _P, _P, _P, c_int, c_int, _P, c_int, _P],
     # tensor-core convolution (include/nslam_nn.h)
     "nslam_conv_igemm": [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int,
                          _P, _P, _P, _P, _P, c_int, _P, _P, c_int, _P],

@@ -188,11 +188,11 @@ static __global__ void fx_flush_kernel(long long* __restrict__ acc, float* __res
 
 // library-owned device scratch, one buffer per (device, slot), grown on demand and zero-filled when (re)allocated
 inline void* ngp_scratch(int slot, size_t bytes) {
-  static void* ptr[64][4] = {};
-  static size_t cap[64][4] = {};
+  static void* ptr[64][5] = {};
+  static size_t cap[64][5] = {};
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64 || slot < 0 || slot >= 4) return nullptr;
+  if (dev < 0 || dev >= 64 || slot < 0 || slot >= 5) return nullptr;
   if (cap[dev][slot] < bytes) {
     if (ptr[dev][slot]) cudaFree(ptr[dev][slot]);
     ptr[dev][slot] = nullptr; cap[dev][slot] = 0;
@@ -202,5 +202,5 @@ inline void* ngp_scratch(int slot, size_t bytes) {
   }
   return ptr[dev][slot];
 }
-enum { NGP_SCRATCH_GRID = 0, NGP_SCRATCH_DW = 1, NGP_SCRATCH_CAM = 2, NGP_SCRATCH_LOSS = 3 };
+enum { NGP_SCRATCH_GRID = 0, NGP_SCRATCH_DW = 1, NGP_SCRATCH_CAM = 2, NGP_SCRATCH_LOSS = 3, NGP_SCRATCH_MESH = 4 };
 

@@ -626,6 +626,50 @@ grid_scatter_kernel(const float* __restrict__ coords, const int* __restrict__ co
   }
 }
 
+// density head of one 128-sample tile, issued by the whole CTA (one warpgroup): hash encode of this thread's point x01
+// (zeros when !act) -> A row -> layer 1 (ReLU) -> layer 2, both on tensor cores against the W1 / W2 images at w_addr.
+// Returns the first output of layer 2 (log density).  The accumulator tile is still read by other threads on return:
+// the caller synchronises before the next tile.  Shared by the occupancy refresh and the mesh lattice.
+__device__ __forceinline__ float density_head_tc(const float x01[3], bool act, const __half2* __restrict__ grid,
+                                                 const LevelInfo& lv, uint32_t a_addr, uint32_t w_addr,
+                                                 unsigned char* arow, float* scr, int tid) {
+  {
+    float enc[ENC_DIM];
+    if (act) {
+      hash_encode(x01, grid, lv, enc);
+    } else {
+#pragma unroll
+      for (int k = 0; k < ENC_DIM; k++) enc[k] = 0.f;
+    }
+    const float z8[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+#pragma unroll
+    for (int c = 0; c < 4; c++) store_row_chunk(arow, tid, c, enc + 8 * c);
+#pragma unroll
+    for (int c = 4; c < 8; c++) store_row_chunk(arow, tid, c, z8);
+  }
+  NGP_TC_SYNC();
+  mma_layer<64>(a_addr, w_addr + PW1, 2, scr, tid);
+  {
+    uint32_t r[32];
+    float v[8];
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      tc::smem_row_ld<32>(scr, SCR_LD, tid, h * 32, r);
+#pragma unroll
+      for (int c = 0; c < 4; c++) {
+#pragma unroll
+        for (int j = 0; j < 8; j++) v[j] = fmaxf(__uint_as_float(r[c * 8 + j]), 0.f);
+        store_row_chunk(arow, tid, h * 4 + c, v);
+      }
+    }
+  }
+  NGP_TC_SYNC();
+  mma_layer<16>(a_addr, w_addr + PW2, 4, scr, tid);
+  uint32_t r[32];
+  tc::smem_row_ld<32>(scr, SCR_LD, tid, 0, r);
+  return __uint_as_float(r[0]);
+}
+
 // occupancy-grid refresh on tensor cores: cell -> jittered point -> hash encode -> density MLP (layers 1-2)
 // -> EMA-max into density[].  Same sampling rule as ngp::density_sample_kernel (csrc/ngp_train.cu).
 __global__ void __launch_bounds__(128)
@@ -662,47 +706,96 @@ density_tc_kernel(const __half2* __restrict__ grid, LevelInfo lv, const unsigned
 #pragma unroll
       for (int k = 0; k < 3; k++) x01[k] = (p[k] - aabb_lo) * inv_extent;
     }
-    {
-      float enc[ENC_DIM];
-      if (actv) {
-        hash_encode(x01, grid, lv, enc);
-      } else {
-#pragma unroll
-        for (int k = 0; k < ENC_DIM; k++) enc[k] = 0.f;
-      }
-      const float z8[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-#pragma unroll
-      for (int c = 0; c < 4; c++) store_row_chunk(arow, tid, c, enc + 8 * c);
-#pragma unroll
-      for (int c = 4; c < 8; c++) store_row_chunk(arow, tid, c, z8);
-    }
-    NGP_TC_SYNC();
-    mma_layer<64>(a_addr, w_addr + PW1, 2, scr, tid);
-    {
-      uint32_t r[32];
-      float v[8];
-#pragma unroll
-      for (int h = 0; h < 2; h++) {
-        tc::smem_row_ld<32>(scr, SCR_LD, tid, h * 32, r);
-#pragma unroll
-        for (int c = 0; c < 4; c++) {
-#pragma unroll
-          for (int j = 0; j < 8; j++) v[j] = fmaxf(__uint_as_float(r[c * 8 + j]), 0.f);
-          store_row_chunk(arow, tid, h * 4 + c, v);
-        }
-      }
-    }
-    NGP_TC_SYNC();
-    mma_layer<16>(a_addr, w_addr + PW2, 4, scr, tid);
-    {
-      uint32_t r[32];
-      tc::smem_row_ld<32>(scr, SCR_LD, tid, 0, r);
-      if (actv) {
-        const float thick = __expf(__uint_as_float(r[0])) * MIN_STEP * s;   // optical thickness of one minimal step
-        density[gi] = fmaxf(density[gi] * decay, thick);
-      }
+    const float o0 = density_head_tc(x01, actv, grid, lv, a_addr, w_addr, arow, scr, tid);
+    if (actv) {
+      const float thick = __expf(o0) * MIN_STEP * s;   // optical thickness of one minimal step
+      density[gi] = fmaxf(density[gi] * decay, thick);
     }
     __syncthreads();
+  }
+}
+
+// ============================================================================================
+// NeRF mesh read-out (Testbed.compute_marching_cubes_mesh).
+//
+// Lattice: point (i,j,k) of [nz,ny,nx] (x fastest) sits at p = lo + h (i,j,k) (fp32, __fmul_rn / __fadd_rn), in the
+// world frame of the training cameras.  Its hash input is x01 = (p - aabb_lo) inv_extent as in density_tc_kernel, its
+// density sigma = __expf(first output of layers 1-2) (density_head_tc), and the kernel writes
+//   field  = thresh - sigma (__fsub_rn): negative inside (sigma > thresh), like a TSDF;
+//   weight = 1 when p is observed, else 0: the occupancy cell of cascade mip_from_pos(p) (the finest cascade whose box
+//            holds p, the one the ray marcher reads there) exists and has density >= 0, i.e. density_mark_kernel saw it
+//            from a training camera.  A point outside every cascade is unobserved.
+// The marching cubes of csrc/tsdf_mesh.cu then run on (field, weight) with min_weight 0, so cubes with an unobserved
+// corner are not meshed; normals point toward +field (lower density, outward).
+__global__ void __launch_bounds__(128)
+mesh_lattice_kernel(const __half2* __restrict__ grid, LevelInfo lv, const unsigned char* __restrict__ packed,
+                    float aabb_lo, float inv_extent, int cascades, const float* __restrict__ density, float3 lo, float h,
+                    int nx, int ny, int nz, float thresh, float* __restrict__ field, float* __restrict__ weight) {
+  extern __shared__ unsigned char smem_raw[];
+  unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  float* scr = reinterpret_cast<float*>(sm + FwdSmem::SCR);
+  const int tid = threadIdx.x;
+  const size_t total = (size_t)nx * ny * nz;
+  const size_t ntiles = (total + 127) / 128;
+  for (int i = tid; i < PW3 / 16; i += 128)          // W1 and W2 images only
+    reinterpret_cast<uint4*>(sm + FwdSmem::W)[i] = reinterpret_cast<const uint4*>(packed)[i];
+  NGP_TC_SYNC();
+  const uint32_t a_addr = tc::smem_u32(sm + FwdSmem::A), w_addr = tc::smem_u32(sm + FwdSmem::W);
+  unsigned char* arow = sm + FwdSmem::A + tid * 128;
+  const size_t NC = (size_t)GRID * GRID * GRID;
+  for (size_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const size_t i = tile * 128 + tid;
+    const bool act = i < total;
+    float x01[3] = {0.5f, 0.5f, 0.5f}, w = 0.f;
+    if (act) {
+      const int ix = (int)(i % nx), iy = (int)((i / nx) % ny), iz = (int)(i / ((size_t)nx * ny));
+      const float p[3] = {__fadd_rn(lo.x, __fmul_rn(h, (float)ix)), __fadd_rn(lo.y, __fmul_rn(h, (float)iy)),
+                          __fadd_rn(lo.z, __fmul_rn(h, (float)iz))};
+#pragma unroll
+      for (int k = 0; k < 3; k++) x01[k] = (p[k] - aabb_lo) * inv_extent;
+      const int mip = mip_from_pos(p, cascades);
+      const int c = cell_index(p, mip);
+      w = (c >= 0 && density[(size_t)mip * NC + c] >= 0.f) ? 1.f : 0.f;
+    }
+    const float o0 = density_head_tc(x01, act, grid, lv, a_addr, w_addr, arow, scr, tid);
+    if (act) {
+      field[i] = __fsub_rn(thresh, __expf(o0));
+      weight[i] = w;
+    }
+    __syncthreads();
+  }
+}
+
+// vertex -> coordinate record of forward_tc_kernel: [x01, dt = 0, d], d = -normal (the surface seen from outside), or
+// (0,0,1) where the normal is 0
+__global__ void mesh_color_records_kernel(const float* __restrict__ vertices, const float* __restrict__ normals, int n,
+                                          float aabb_lo, float inv_extent, float* __restrict__ coords) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float* v = vertices + 3 * (size_t)i;
+  const float* nr = normals + 3 * (size_t)i;
+  const bool none = nr[0] == 0.f && nr[1] == 0.f && nr[2] == 0.f;
+  float* c = coords + 7 * (size_t)i;
+#pragma unroll
+  for (int k = 0; k < 3; k++) c[k] = (v[k] - aabb_lo) * inv_extent;
+  c[3] = 0.f;
+  c[4] = none ? 0.f : -nr[0];
+  c[5] = none ? 0.f : -nr[1];
+  c[6] = none ? 1.f : -nr[2];
+}
+
+// network rgb -> vertex colour; srgb: the inverse of the ingest's sRGB -> linear curve (ingest_image_kernel,
+// csrc/ngp_train.cu: s > 0.04045 ? ((s + 0.055) / 1.055)^2.4 : s / 12.92)
+__global__ void mesh_color_store_kernel(const float4* __restrict__ rgbsigma, int n, int srgb, float* __restrict__ colors) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float4 o = rgbsigma[i];
+  const float l[3] = {o.x, o.y, o.z};
+#pragma unroll
+  for (int k = 0; k < 3; k++) {
+    float c = l[k];
+    if (srgb) c = c > 0.0031308f ? __fsub_rn(__fmul_rn(1.055f, powf(c, 1.f / 2.4f)), 0.055f) : __fmul_rn(c, 12.92f);
+    colors[3 * (size_t)i + k] = c;
   }
 }
 
@@ -845,6 +938,60 @@ int nslam_ngp_density_sample_tc(const nslam_ngp_model* m, const void* packed, in
                                                               0.5f - 0.5f * m->aabb_scale, 1.f / m->aabb_scale, m->cascades,
                                                               n_per_cascade, seed, decay, m->density);
   return (int)cudaGetLastError();
+}
+
+/* NeRF mesh lattice: field / weight [nz,ny,nx] fp32 (DEVICE) of the lattice lo3_host + h (i,j,k) (see mesh_lattice_kernel) */
+int nslam_ngp_mesh_lattice(const nslam_ngp_model* m, const void* packed, const float* lo3_host, float h, int nx, int ny,
+                           int nz, float thresh, float* field, float* weight, int num_sms, void* stream) {
+  using namespace ngp;
+  if (nx <= 0 || ny <= 0 || nz <= 0) return (int)cudaErrorInvalidValue;
+  LevelInfo lv;
+  for (int l = 0; l < N_LEVELS; l++) {
+    lv.scale[l] = m->scale[l]; lv.res[l] = m->res[l]; lv.size[l] = m->size[l];
+    lv.offset[l] = m->offset[l]; lv.dense[l] = m->dense[l];
+  }
+  const int smem = FwdSmem::TOTAL + 1024;
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(mesh_lattice_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return (int)e;
+    configured = true;
+  }
+  const size_t tiles = ((size_t)nx * ny * nz + 127) / 128;
+  const int grid = (int)(tiles < (size_t)4 * num_sms ? tiles : (size_t)4 * num_sms);
+  mesh_lattice_kernel<<<grid, 128, smem, (cudaStream_t)stream>>>((const __half2*)m->grid_half, lv, (const unsigned char*)packed,
+                                                                 0.5f - 0.5f * m->aabb_scale, 1.f / m->aabb_scale, m->cascades,
+                                                                 m->density, make_float3(lo3_host[0], lo3_host[1], lo3_host[2]),
+                                                                 h, nx, ny, nz, thresh, field, weight);
+  return (int)cudaGetLastError();
+}
+
+/* NeRF mesh vertex colours: colors [n,3] = network radiance at vertices [n,3] seen along -normals [n,3] (DEVICE), through
+ * the tensor-core forward in chunks of library-owned scratch; srgb != 0: encoded with the inverse of the ingest's curve */
+int nslam_ngp_mesh_colors(const nslam_ngp_model* m, const void* packed, const float* vertices, const float* normals, int n,
+                          int srgb, float* colors, int num_sms, void* stream) {
+  using namespace ngp;
+  if (n < 0) return (int)cudaErrorInvalidValue;
+  if (n == 0) return 0;
+  constexpr int CHUNK = 1 << 18;
+  const int cap = n < CHUNK ? n : CHUNK;
+  float* rgbsigma = (float*)ngp_scratch(NGP_SCRATCH_MESH, (size_t)cap * 11 * sizeof(float));   // [cap,4] then [cap,7]
+  if (!rgbsigma) return (int)cudaErrorMemoryAllocation;
+  float* coords = rgbsigma + (size_t)cap * 4;
+  cudaStream_t st = (cudaStream_t)stream;
+  for (int base = 0; base < n; base += CHUNK) {
+    const int c = n - base < CHUNK ? n - base : CHUNK;
+    mesh_color_records_kernel<<<(c + 255) / 256, 256, 0, st>>>(vertices + 3 * (size_t)base, normals + 3 * (size_t)base, c,
+                                                               0.5f - 0.5f * m->aabb_scale, 1.f / m->aabb_scale, coords);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return (int)e;
+    int r = nslam_ngp_forward_tc(m, packed, coords, nullptr, c, c, rgbsigma, nullptr, num_sms, stream);
+    if (r) return r;
+    mesh_color_store_kernel<<<(c + 255) / 256, 256, 0, st>>>((const float4*)rgbsigma, c, srgb, colors + 3 * (size_t)base);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return (int)e;
+  }
+  return 0;
 }
 
 }  // extern "C"

@@ -125,7 +125,8 @@ struct DenseVox {
   }
   __device__ __forceinline__ float t(int i, int j, int k) const { return tsdf[idx(i, j, k)]; }
   __device__ __forceinline__ float w(int i, int j, int k) const { return weight[idx(i, j, k)]; }
-  __device__ __forceinline__ float c(int i, int j, int k, int ch) const { return color[idx(i, j, k) * 3 + ch]; }
+  // color == nullptr: a volume without colours (the NeRF mesh lattice), colour 0
+  __device__ __forceinline__ float c(int i, int j, int k, int ch) const { return color ? color[idx(i, j, k) * 3 + ch] : 0.f; }
   __device__ __forceinline__ DenseVox bind(size_t v, int& i, int& j, int& k) const {
     i = (int)(v % nx);
     j = (int)((v / nx) % ny);

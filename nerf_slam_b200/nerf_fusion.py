@@ -2,6 +2,7 @@
 
 Same surface: NerfFusion(name, args, device) .fuse(data_packets) .stop_condition()
               .process_slam / .process_data / .send_data / .fit_volume / .fit_volume_once / .eval_gt_traj
+Beyond the reference: `build_mesh` reads the trained NeRF out as a coloured marching-cubes mesh (pyngp.Testbed.marching_cubes).
 Differences by design: the SLAM packet's CUDA tensors go straight into the trainer's device slots
 (sRGB->linear, premultiply, 1/idepth fused in one kernel) — the reference converts on the GPU,
 copies to the CPU, to numpy, into pyngp and back to the GPU ("extremely slow", :209).
@@ -76,6 +77,9 @@ class NerfFusion:
         self.evaluate = bool(getattr(args, "eval", False))
         self.eval_every_iters = 200
         self.results = []
+        # the training colours are linear (process_slam, process_data "metric") or sRGB values / 255 (process_data
+        # "reference"); build_mesh hands its vertex colours back in the images' own encoding
+        self.linear_training_colors = True
         self.fit_volume_once()
 
     # ------------------------------------------------------------------ B1
@@ -92,6 +96,7 @@ class NerfFusion:
         depths_cov_up = slam["cam0_depths_cov_up"]
         calib = slam["calibs"][0]
         assert images.dtype == torch.uint8 and idepths_up.dtype == torch.float32
+        self.linear_training_colors = True                          # sRGB -> linear in the ingest kernel
         if self.mask_type == "raw":
             depths_cov_up = torch.ones_like(depths_cov_up)
         elif self.mask_type == "ours_w_thresh":
@@ -140,7 +145,9 @@ class NerfFusion:
         c2w = np.linalg.inv(np.asarray(packet["poses"], np.float64))
         dep = np.asarray(packet["depths"]).astype(np.float32)
         intr = calib.camera_model.numpy()
-        if getattr(self, "gt_fit_convention", "reference") == "reference":
+        reference = getattr(self, "gt_fit_convention", "reference") == "reference"
+        self.linear_training_colors = not reference
+        if reference:
             scale, offset = get_scale_and_offset(calib.aabb)
             c2w[:, :3, 3] = c2w[:, :3, 3] * scale + offset
             rgba = np.asarray(packet["images"]).astype(np.float32) / 255.0
@@ -193,6 +200,14 @@ class NerfFusion:
         if self.evaluate and self.total_iters % self.eval_every_iters == 0 and self.ngp.rgba is not None:
             self.eval_gt_traj()
         self.total_iters += 1
+
+    # ------------------------------------------------------------------ mesh read-out
+    def build_mesh(self, resolution=256, thresh=2.5, aabb=None):
+        """marching-cubes mesh of the NeRF's density level set sigma = thresh (pyngp.Testbed.marching_cubes) -> TsdfMesh of
+        device tensors in the training cameras' world frame, or None when no triangle results (as TsdfFusion.build_mesh).
+        Vertex colours come back in the encoding of the training images: sRGB when the ingest linearised them
+        (process_slam, process_data with gt_fit_convention "metric"), the network's values for the reference convention."""
+        return self.ngp.marching_cubes(resolution, aabb, thresh, srgb=self.linear_training_colors)
 
     # ------------------------------------------------------------------ B4
     def eval_gt_traj(self, stride=2):

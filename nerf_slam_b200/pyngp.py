@@ -12,6 +12,8 @@ fork's python module (SURVEY.md §8b "pyngp surface used"):
   .frame()  .loss  .elapsed_training_time  .apply_camera_smoothing(ms)
   .background_color .snap_to_pixel_centers .nerf.rendering_min_transmittance .camera_matrix
   .render_mode .set_camera_to_training_view(i) .render(w, h, spp, linear, fps=)
+  .compute_marching_cubes_mesh(resolution, aabb, thresh) .compute_and_save_marching_cubes_mesh(filename, ...)
+    (instant-ngp's mesh export; not called by fusion/nerf_fusion.py)
 
 plus a device-side fast path (`update_training_images_device`) that takes the SLAM packet's CUDA
 tensors directly (no CPU round trip, cf. fusion/nerf_fusion.py:198-223).
@@ -79,6 +81,66 @@ def level_table(aabb_scale):
         rows.append((float(np.float32(scale)), res, n, off, int(res ** 3 <= n)))
         off += n
     return rows, off
+
+
+INT32_MAX = (1 << 31) - 1
+
+
+def mesh_lattice(resolution, aabb, aabb_scale):
+    """lattice of the NeRF mesh read-out -> (lo float32 [3], h float32, (nx, ny, nz)); point (i,j,k) sits at lo + h (i,j,k)
+    in the training cameras' world frame.
+
+    `resolution`: int, or a 3-sequence whose maximum is used = number of points along the longest side of the box.
+    `aabb`: BoundingBox or [[min],[max]]; None = the training box [0.5 -/+ aabb_scale / 2]^3; clipped to that box (the hash
+    grid covers nothing outside it).  h = longest extent / (resolution - 1), n_a = floor(extent_a / h) + 1.  ValueError for
+    resolution < 2, an empty box, or a lattice whose worst-case vertex / triangle count overflows int32 (about 750^3)."""
+    res = int(max(resolution)) if np.ndim(resolution) else int(resolution)
+    if res < 2:
+        raise ValueError(f"mesh resolution must be at least 2, not {resolution!r}")
+    box = np.array([0.5 - 0.5 * aabb_scale, 0.5 + 0.5 * aabb_scale], np.float64)
+    if aabb is None:
+        lo, hi = np.full(3, box[0]), np.full(3, box[1])
+    else:
+        mn, mx = (aabb.min, aabb.max) if isinstance(aabb, BoundingBox) else aabb
+        lo = np.maximum(np.asarray(mn, np.float64).reshape(3), box[0])
+        hi = np.minimum(np.asarray(mx, np.float64).reshape(3), box[1])
+    ext = hi - lo
+    if not np.all(ext > 0):                          # also rejects NaN
+        raise ValueError(f"empty mesh box {lo.tolist()} .. {hi.tolist()} inside the training box {box.tolist()}")
+    h = float(ext.max()) / (res - 1)
+    dims = tuple(min(res, int(np.floor(e / h + 1e-9)) + 1) for e in ext)
+    n = dims[0] * dims[1] * dims[2]
+    cubes = (dims[0] - 1) * (dims[1] - 1) * (dims[2] - 1)
+    if 3 * n > INT32_MAX or 5 * cubes > INT32_MAX:
+        raise ValueError(f"mesh lattice {dims} too large: its worst-case vertex / triangle count overflows int32")
+    return lo.astype(np.float32), np.float32(h), dims
+
+
+class _MeshKernels:
+    """the three device passes of Testbed.marching_cubes (tests substitute a host restatement)"""
+
+    def lattice(self, tb, lo, h, dims, thresh):
+        """-> field, weight [nz,ny,nx] (see nslam_ngp_mesh_lattice)"""
+        nx, ny, nz = dims
+        field = torch.empty(nz, ny, nx, dtype=torch.float32, device=tb.device)
+        weight = torch.empty_like(field)
+        lo = np.ascontiguousarray(lo, np.float32)
+        _lib.check(_lib.load().nslam_ngp_mesh_lattice(ctypes.byref(tb.model), _lib.ptr(tb.packed), lo.ctypes.data, float(h),
+                                                      nx, ny, nz, float(thresh), _lib.ptr(field), _lib.ptr(weight),
+                                                      tb.num_sms, _lib.stream_ptr()), "ngp_mesh_lattice")
+        return field, weight
+
+    def mesh(self, field, weight, lo, h):
+        """marching cubes over the cubes whose 8 corners are observed -> TsdfMesh (colours 0) or None"""
+        from .tsdf_fusion import mesh_dense
+        return mesh_dense(field, weight, None, lo, h, 0.0)
+
+    def colors(self, tb, mesh, srgb):
+        """mesh.vertex_colors <- the network's radiance at the vertices, seen from outside"""
+        v, n = mesh.vertices, mesh.vertex_normals
+        _lib.check(_lib.load().nslam_ngp_mesh_colors(ctypes.byref(tb.model), _lib.ptr(tb.packed), _lib.ptr(v), _lib.ptr(n),
+                                                     int(v.shape[0]), int(bool(srgb)), _lib.ptr(mesh.vertex_colors),
+                                                     tb.num_sms, _lib.stream_ptr()), "ngp_mesh_colors")
 
 
 class _Training:
@@ -405,6 +467,49 @@ class Testbed:
 
     def apply_camera_smoothing(self, ms):
         pass
+
+    # ---------------------------------------------------------------- mesh read-out
+    mesh_kernels = _MeshKernels()
+
+    def marching_cubes(self, resolution=256, aabb=None, thresh=2.5, srgb=False):
+        """marching-cubes mesh of the density field -> TsdfMesh of device tensors, or None when no triangle results.
+
+        The density sigma is sampled on the lattice of `mesh_lattice(resolution, aabb, aabb_scale)`; the surface is the
+        level set sigma = thresh (inside: sigma > thresh).  Only cubes whose 8 corners lie in occupancy cells seen by a
+        training camera are meshed.  Normals are unit, toward lower density (outward), triangles wound outward.  Vertex
+        colours are the network's radiance at the vertex seen along -normal, i.e. from outside: linear as the network
+        outputs them, or sRGB-encoded with `srgb` (the inverse of the ingest's sRGB -> linear curve).  Positions are in
+        the training cameras' world frame (the SLAM world frame for process_slam).  The density and colours always come
+        from the tensor-core network (the packed fp16 weights), whatever `mlp_backend` is."""
+        lo, h, dims = mesh_lattice(resolution, aabb, self.aabb_scale)
+        k = self.mesh_kernels
+        field, weight = k.lattice(self, lo, h, dims, thresh)
+        mesh = k.mesh(field, weight, lo, h)
+        del field, weight                                # 8 B per lattice point, freed before the colour pass
+        if mesh is not None:
+            k.colors(self, mesh, srgb)
+        return mesh
+
+    def compute_marching_cubes_mesh(self, resolution=256, aabb=None, thresh=2.5):
+        """instant-ngp's Testbed.compute_marching_cubes_mesh -> {"V": [V,3] float32, "N": [V,3] unit normals, "C": [V,3]
+        linear colours, "F": [T,3] int32}, numpy; empty arrays when no triangle results.  See `marching_cubes` (the
+        tensor-core network is used whatever `mlp_backend` is)."""
+        mesh = self.marching_cubes(resolution, aabb, thresh)
+        if mesh is None:
+            z = np.zeros((0, 3), np.float32)
+            return {"V": z, "N": z.copy(), "C": z.copy(), "F": np.zeros((0, 3), np.int32)}
+        return {"V": mesh.vertices.cpu().numpy(), "N": mesh.vertex_normals.cpu().numpy(),
+                "C": mesh.vertex_colors.cpu().numpy(), "F": mesh.triangles.cpu().numpy().astype(np.int32)}
+
+    def compute_and_save_marching_cubes_mesh(self, filename, resolution=256, aabb=None, thresh=2.5):
+        """instant-ngp's Testbed.compute_and_save_marching_cubes_mesh: `marching_cubes` written as a binary PLY
+        (TsdfMesh.write_ply; linear colours); an empty mesh when no triangle results"""
+        from .tsdf_fusion import TsdfMesh
+        mesh = self.marching_cubes(resolution, aabb, thresh)
+        if mesh is None:
+            z = torch.zeros(0, 3)
+            mesh = TsdfMesh(z, torch.zeros(0, 3, dtype=torch.int32), z, z)
+        mesh.write_ply(filename)
 
     # ---------------------------------------------------------------- rendering
     def set_camera_to_training_view(self, i):

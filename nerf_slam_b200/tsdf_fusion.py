@@ -63,6 +63,37 @@ class TsdfMesh:
             f.write(ft.tobytes())
 
 
+def mesh_dense(tsdf, weight, color, origin, voxel_size, min_weight):
+    """marching cubes (csrc/tsdf_mesh.cu) over a dense [nz,ny,nx] volume whose voxel (i,j,k) sits at origin + voxel_size *
+    (i,j,k), over the cubes whose 8 corners have weight > min_weight -> TsdfMesh of device tensors, or None when there is
+    no triangle.  `color` [nz,ny,nx,3] on the u8 scale, or None for a volume without colours (vertex colours 0).  One host
+    read of the three counts sizes the outputs."""
+    lib = _lib.load()
+    nz, ny, nx = tsdf.shape
+    dev = tsdf.device
+    org = np.ascontiguousarray(np.asarray(origin, np.float32))
+    n_scratch = np.zeros(1, np.int64)
+    _lib.check(lib.nslam_tsdf_mesh_plan(nx, ny, nz, n_scratch.ctypes.data), "tsdf_mesh_plan")
+    scratch = torch.empty(int(n_scratch[0]), dtype=torch.int32, device=dev)
+    mw = float(min_weight)
+    with _lib.fixed_stream():
+        _lib.check(lib.nslam_tsdf_mesh_count(_lib.ptr(tsdf), _lib.ptr(weight), nx, ny, nz, mw, _lib.ptr(scratch),
+                                             _lib.stream_ptr()), "tsdf_mesh_count")
+        n_vert, n_tri, n_active = scratch[:3].tolist()
+        if n_tri == 0:
+            return None
+        active = torch.empty(n_active, 4, dtype=torch.int32, device=dev)
+        verts = torch.empty(n_vert, 3, dtype=torch.float32, device=dev)
+        cols = torch.empty(n_vert, 3, dtype=torch.float32, device=dev)
+        nrms = torch.empty(n_vert, 3, dtype=torch.float32, device=dev)
+        tris = torch.empty(n_tri, 3, dtype=torch.int32, device=dev)
+        _lib.check(lib.nslam_tsdf_mesh_emit(
+            _lib.ptr(tsdf), _lib.ptr(weight), _lib.ptr(color), nx, ny, nz, org.ctypes.data, float(voxel_size), mw,
+            _lib.ptr(scratch), n_active, _lib.ptr(active), _lib.ptr(verts), _lib.ptr(cols), _lib.ptr(nrms), _lib.ptr(tris),
+            _lib.stream_ptr()), "tsdf_mesh_emit")
+    return TsdfMesh(verts, tris, cols, nrms)
+
+
 def depth_l1_cm(rendered_depth, gt_depth):
     """depth error of one view (:466-474): the last 8 rows and columns dropped, the rendering scaled by the ratio of the
     means, |error| clamped at 2.0, mean x 100 (cm)"""
@@ -288,29 +319,7 @@ class TsdfFusion:
         when there is no triangle.  One host read of the three counts sizes the outputs."""
         if self.volume is not None:
             return self.volume.build_mesh(min_weight_for_mesh)
-        lib = _lib.load()
-        nz, ny, nx = self.tsdf.shape
-        dev = self.tsdf.device
-        n_scratch = np.zeros(1, np.int64)
-        _lib.check(lib.nslam_tsdf_mesh_plan(nx, ny, nz, n_scratch.ctypes.data), "tsdf_mesh_plan")
-        scratch = torch.empty(int(n_scratch[0]), dtype=torch.int32, device=dev)
-        mw = float(min_weight_for_mesh)
-        with _lib.fixed_stream():
-            _lib.check(lib.nslam_tsdf_mesh_count(_lib.ptr(self.tsdf), _lib.ptr(self.weight), nx, ny, nz, mw, _lib.ptr(scratch),
-                                                 _lib.stream_ptr()), "tsdf_mesh_count")
-            n_vert, n_tri, n_active = scratch[:3].tolist()
-            if n_tri == 0:
-                return None
-            active = torch.empty(n_active, 4, dtype=torch.int32, device=dev)
-            verts = torch.empty(n_vert, 3, dtype=torch.float32, device=dev)
-            cols = torch.empty(n_vert, 3, dtype=torch.float32, device=dev)
-            nrms = torch.empty(n_vert, 3, dtype=torch.float32, device=dev)
-            tris = torch.empty(n_tri, 3, dtype=torch.int32, device=dev)
-            _lib.check(lib.nslam_tsdf_mesh_emit(
-                _lib.ptr(self.tsdf), _lib.ptr(self.weight), _lib.ptr(self.color), nx, ny, nz, self.origin.ctypes.data,
-                float(self.voxel_size), mw, _lib.ptr(scratch), n_active, _lib.ptr(active), _lib.ptr(verts), _lib.ptr(cols),
-                _lib.ptr(nrms), _lib.ptr(tris), _lib.stream_ptr()), "tsdf_mesh_emit")
-        return TsdfMesh(verts, tris, cols, nrms)
+        return mesh_dense(self.tsdf, self.weight, self.color, self.origin, self.voxel_size, min_weight_for_mesh)
 
     def render_volume(self, packet, intrinsics, min_weight_for_render, max_depth_sigma_thresh, evaluate=False):
         """:319-484: ray-cast depth and colour at every keyframe of the packet -> (depth [n,H,W], colour [n,H,W,3] in [0,1]);
