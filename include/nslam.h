@@ -189,6 +189,27 @@ int nslam_tsdf_blocks_raycast(const float* tsdf, const float* weight, const floa
                               float max_depth, float sdf_trunc, float min_weight, float* depth, float* color_out,
                               float* weight_out, float* normal_out, void* stream);
 
+/* Coloured point cloud of the SLAM keyframe map (csrc/point_cloud.cu; rules at its head).  Replaces the reference GUI's
+ * get_depth_masks + build_pcls (gui/open3d_gui.py:289-299, 646-678: Open3D's create_from_rgbd_image per keyframe) and
+ * Open3D's PointCloud.voxel_down_sample.  Cloud: _scratch -> _count (classify + scan, *total = kept points, DEVICE) ->
+ * _emit (points / colors [total,3] fp32) with the same inputs and scratch.  views = droid_backends.depth_filter's
+ * counter [n,H,W] or NULL (no multi-view filter), min_views 1..6.  Downsampling: _voxel_scratch -> _voxel_sort
+ * (*n_voxels, DEVICE) -> _voxel_reduce (means and counts).  All tensors DEVICE; n H W <= INT32_MAX. */
+int nslam_point_cloud_scratch(int n, int H, int W, long long* bytes);
+int nslam_point_cloud_count(const float* idepth_up, const float* depth_cov_up, const float* views, int min_views, int n,
+                            int H, int W, float max_depth, float max_depth_sigma, void* scratch, long long scratch_bytes,
+                            int* total, void* stream);
+int nslam_point_cloud_emit(const float* cam_T_world_tq, const float* idepth_up, const float* depth_cov_up, const float* views,
+                           int min_views, const unsigned char* rgb_chw, const float* intr4, int n, int H, int W,
+                           float max_depth, float max_depth_sigma, const void* scratch, long long scratch_bytes,
+                           float* points, float* colors, void* stream);
+int nslam_point_cloud_voxel_scratch(int n_points, long long* bytes);
+int nslam_point_cloud_voxel_sort(const float* points, int n_points, float voxel_size, void* scratch, long long scratch_bytes,
+                                 int* n_voxels, void* stream);
+int nslam_point_cloud_voxel_reduce(const float* points, const float* colors, int n_points, const void* scratch,
+                                   long long scratch_bytes, int n_voxels, float* out_points, float* out_colors,
+                                   int* out_counts, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -98,6 +98,13 @@ _SIGNATURES = {
     "nslam_tsdf_blocks_mesh_emit": [_P, _P, _P, _P, _P, c_int, c_float, c_float, _P, c_int, _P, _P, _P, _P, _P, _P],
     "nslam_tsdf_blocks_raycast": [_P, _P, _P, _P, _P, _P, c_int, c_float, _P, c_int, c_int, c_int, _P, c_float, c_float,
                                   c_float, c_float, _P, _P, _P, _P, _P],
+    "nslam_point_cloud_scratch": [c_int, c_int, c_int, _P],
+    "nslam_point_cloud_count": [_P, _P, _P, c_int, c_int, c_int, c_int, c_float, c_float, _P, ctypes.c_longlong, _P, _P],
+    "nslam_point_cloud_emit": [_P, _P, _P, _P, c_int, _P, _P, c_int, c_int, c_int, c_float, c_float, _P, ctypes.c_longlong,
+                               _P, _P, _P],
+    "nslam_point_cloud_voxel_scratch": [c_int, _P],
+    "nslam_point_cloud_voxel_sort": [_P, c_int, c_float, _P, ctypes.c_longlong, _P, _P],
+    "nslam_point_cloud_voxel_reduce": [_P, _P, c_int, _P, ctypes.c_longlong, c_int, _P, _P, _P, _P],
     "nslam_ba_reduced_camera_matrix": [ctypes.POINTER(BAGraph), ctypes.POINTER(BABuffers), _P],
     "nslam_ba_tile_pixels": [],
     "nslam_ba_solve": [_P, _P, c_int, c_int, _P, c_float, c_float, c_float, _P, _P, _P, _P, _P],

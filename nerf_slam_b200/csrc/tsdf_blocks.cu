@@ -41,14 +41,7 @@
 
 namespace nslam {
 
-constexpr unsigned long long kEmpty = ~0ull;     // empty hash slot / dropped key (packed keys are < 2^63)
-constexpr int kBias = 1 << 20;
-
-__device__ __forceinline__ unsigned long long pack_block(long long bx, long long by, long long bz) {
-  return (unsigned long long)(bx + kBias) | ((unsigned long long)(by + kBias) << 21) | ((unsigned long long)(bz + kBias) << 42);
-}
-
-__device__ __forceinline__ bool block_in_range(double q) { return q >= -(double)kBias && q < (double)kBias; }
+// block keys: pack_block / block_in_range / kEmpty in tsdf_rules.cuh
 
 __device__ __forceinline__ unsigned hash_slot(unsigned long long k, unsigned mask) {
   k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;

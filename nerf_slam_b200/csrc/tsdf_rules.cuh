@@ -41,6 +41,19 @@ __device__ __forceinline__ float tsdf_pixel_depth(const TsdfFrame& f, size_t pix
   return depth;
 }
 
+// ------------------------------------------------------------------------------------------------------- lattice keys
+// A cell (x,y,z) of an integer lattice (the 16^3 blocks of tsdf_blocks.cu, the voxels of point_cloud.cu's downsampling)
+// is a 63-bit key (x + 2^20) | (y + 2^20) << 21 | (z + 2^20) << 42, so ascending keys run z-major.  Cells outside
+// [-2^20, 2^20)^3 are dropped, never wrapped: test every coordinate with block_in_range first.
+constexpr unsigned long long kEmpty = ~0ull;     // empty hash slot / dropped key (packed keys are < 2^63)
+constexpr int kBias = 1 << 20;
+
+__device__ __forceinline__ unsigned long long pack_block(long long bx, long long by, long long bz) {
+  return (unsigned long long)(bx + kBias) | ((unsigned long long)(by + kBias) << 21) | ((unsigned long long)(bz + kBias) << 42);
+}
+
+__device__ __forceinline__ bool block_in_range(double q) { return q >= -(double)kBias && q < (double)kBias; }
+
 // One voxel, one keyframe (reference fusion/tsdf_fusion.py:231-296).  (wxf, wyf, wzf) = the voxel's fp32 world
 // coordinate, promoted to fp64 with the pose and the intrinsics for the projection.  tsdf / weight point at the voxel,
 // color at its 3 channels.

@@ -1000,3 +1000,23 @@ class RaftVisualFrontend:
                "kf_idx_to_f_idx": dict(self.kf_idx_to_f_idx), "is_last_frame": batch["is_last_frame"]}
         self.viz_idx[:] = False
         return out
+
+    def point_cloud(self, mask_type="uncertainty", voxel_size=None, filter_thresh=None, min_views=2, max_depth=6.0,
+                    max_depth_sigma=10.0):
+        """every keyframe the buffer holds as one coloured point cloud (point_cloud.build_point_cloud; the reference
+        GUI's build_pcls, gui/open3d_gui.py:646-678, whose defaults max_depth 6 and max_depth_sigma_thresh 10 are kept)
+        -> PointCloud, or None.  Reads the arenas in place (cam0_T_world, cam0_idepths_up, cam0_depths_cov_up,
+        cam0_images, dsf * cam0_intrinsics[0]) on the current stream; the only host reads are the point and voxel
+        counts.  mask_type "uncertainty" (the demo's --mask_type ours) or "uniform"."""
+        from .point_cloud import build_point_cloud
+        if mask_type not in ("uncertainty", "uniform"):
+            raise ValueError(f"Unknown depth mask type: {mask_type}")
+        if not hasattr(self, "cam0_T_world"):
+            return None
+        n = min(self.kf_idx + 1 if self.stop else self.kf_idx, self.buffer)    # slot kf_idx is the next keyframe's until stop
+        packet = {"cam0_poses": self.cam0_T_world[:n], "cam0_idepths_up": self.cam0_idepths_up[:n],
+                  "cam0_depths_cov_up": self.cam0_depths_cov_up[:n] if mask_type == "uncertainty" else None,
+                  "cam0_images": self.cam0_images[:n]}
+        return build_point_cloud(packet, self.dsf * self.cam0_intrinsics[0], max_depth=max_depth,
+                                 max_depth_sigma=max_depth_sigma, filter_thresh=filter_thresh, min_views=min_views,
+                                 voxel_size=voxel_size)

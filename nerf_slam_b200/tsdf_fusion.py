@@ -4,7 +4,7 @@ sm_90a voxel grid.
 Same surface: TsdfFusion(name, args, device)  .fuse(data_packets)  .stop_condition()
               .handle_slam_packet / .handle_gui_packet / .update_history / .get_history_packet / .get_depth_masks /
               .build_volume / .rebuild_volume / .reset_volume / .build_mesh / .render_volume / .evaluate_metrics
-              (the Open3D GUI itself is out of scope)
+              .build_point_cloud (the GUI's point clouds; the Open3D GUI itself is out of scope)
 name "tsdf": uniform weights; "sigma": weights 1 / sqrt(depth variance) from the SLAM packet's covariances
 (Rosinol22wacv; tsdf_fusion.py:46-49,196).
 
@@ -31,6 +31,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .point_cloud import build_point_cloud as _build_point_cloud, write_binary_ply
 from .tsdf_blocks import VoxelBlockVolume
 
 
@@ -45,22 +46,13 @@ class TsdfMesh:
 
     def write_ply(self, path):
         """binary little-endian PLY: float x y z nx ny nz red green blue (colours in [0,1]), int32 vertex indices"""
-        v = self.vertices.detach().float().cpu().numpy()
-        vt = np.empty(v.shape[0], [(k, "<f4") for k in ("x", "y", "z", "nx", "ny", "nz", "red", "green", "blue")])
-        for k, (src, c) in zip(vt.dtype.names, [(v, 0), (v, 1), (v, 2)] +
-                               [(self.vertex_normals.detach().float().cpu().numpy(), c) for c in range(3)] +
-                               [(self.vertex_colors.detach().float().cpu().numpy(), c) for c in range(3)]):
-            vt[k] = src[:, c]
-        t = self.triangles.detach().cpu().numpy().astype("<i4")
-        ft = np.empty(t.shape[0], [("n", "u1"), ("v", "<i4", (3,))])
-        ft["n"], ft["v"] = 3, t
-        head = ["ply", "format binary_little_endian 1.0", f"element vertex {v.shape[0]}"] + \
-               [f"property float {k}" for k in vt.dtype.names] + \
-               [f"element face {t.shape[0]}", "property list uchar int vertex_indices", "end_header"]
-        with open(path, "wb") as f:
-            f.write(("\n".join(head) + "\n").encode("ascii"))
-            f.write(vt.tobytes())
-            f.write(ft.tobytes())
+        arrays = [(("x", "y", "z"), self.vertices), (("nx", "ny", "nz"), self.vertex_normals),
+                  (("red", "green", "blue"), self.vertex_colors)]
+        cols = []
+        for names, t in arrays:
+            a = t.detach().float().cpu().numpy()
+            cols += [(k, a[:, i]) for i, k in enumerate(names)]
+        write_binary_ply(path, cols, self.triangles.detach().cpu().numpy())
 
 
 def mesh_dense(tsdf, weight, color, origin, voxel_size, min_weight):
@@ -191,6 +183,14 @@ class TsdfFusion:
                 output = {"mesh": mesh}
             else:
                 print("Could not build a mesh...")
+        pcl_opts = packet.get("build_pcl")
+        if pcl_opts is not None and pcl_opts is not False:
+            # {"build_pcl": {}} or True; options: voxel_size, filter_thresh, min_views
+            pcl = self.build_point_cloud(**(pcl_opts if isinstance(pcl_opts, dict) else {}))
+            if pcl is not None:
+                output = dict(output or {}, pcl=pcl)
+            else:
+                print("Could not build a point cloud...")
         if packet.get("rebuild_volume"):
             self.rebuild_volume()
         if packet.get("eval_metrics"):
@@ -320,6 +320,26 @@ class TsdfFusion:
         if self.volume is not None:
             return self.volume.build_mesh(min_weight_for_mesh)
         return mesh_dense(self.tsdf, self.weight, self.color, self.origin, self.voxel_size, min_weight_for_mesh)
+
+    def build_point_cloud(self, voxel_size=None, filter_thresh=None, min_views=2):
+        """the GUI's build_pcls(None), "rebuild from history" (gui/open3d_gui.py:646-678): every keyframe of the history
+        as one coloured point cloud (point_cloud.build_point_cloud) with this fusion's depth_mask_type,
+        max_depth_sigma_thresh, max_depth and intrinsics -> PointCloud, or None when there is no history or no point.
+        Reads the history, not the volume, so it works for both tsdf_volume modes."""
+        if not self.history:
+            return None
+        packet = self.get_history_packet()
+        if self.depth_mask_type == "uniform":
+            packet["cam0_depths_cov_up"] = None
+        elif self.depth_mask_type != "uncertainty":
+            raise NotImplementedError(f"Unknown depth mask type: {self.depth_mask_type}")
+        dev = packet["cam0_idepths_up"].device
+        for k in ("cam0_poses", "cam0_idepths_up", "cam0_depths_cov_up"):
+            if packet[k] is not None:
+                packet[k] = packet[k].to(dev, torch.float32).contiguous()
+        return _build_point_cloud(packet, self.intrinsics, max_depth=self.max_depth,
+                                  max_depth_sigma=self.max_depth_sigma_thresh, filter_thresh=filter_thresh,
+                                  min_views=min_views, voxel_size=voxel_size)
 
     def render_volume(self, packet, intrinsics, min_weight_for_render, max_depth_sigma_thresh, evaluate=False):
         """:319-484: ray-cast depth and colour at every keyframe of the packet -> (depth [n,H,W], colour [n,H,W,3] in [0,1]);
