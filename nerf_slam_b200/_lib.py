@@ -230,12 +230,15 @@ def ptr(t):
 def h2d(a, device, dtype=None):
     """numpy array (or list) -> device tensor through PINNED memory with a non-blocking copy.
     `torch.as_tensor(ndarray, device=...)` copies from pageable memory, which makes the CUDA runtime
-    synchronise the stream before every copy (one hidden device sync per small index upload)."""
+    synchronise the stream before every copy (one hidden device sync per small index upload).
+    A CPU `device` gets the host tensor itself (no copy)."""
     import numpy as np
     import torch
     t = torch.from_numpy(np.ascontiguousarray(a))
     if dtype is not None and t.dtype != dtype:
         t = t.to(dtype)
+    if torch.device(device).type == "cpu":
+        return t
     if t.numel() == 0:
         return torch.empty(t.shape, dtype=t.dtype, device=device)
     return t.pin_memory().to(device, non_blocking=True)

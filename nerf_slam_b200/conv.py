@@ -230,20 +230,15 @@ class UpdateOperatorTC:
         """UpdateModule.forward's own argument/return convention (droid_net.py:118-150) on top of the fused
         operator — used by the parity tests: motion [E,4,ht,wd] (|.| < 64) is turned into the coordinate
         tensors it is derived from in the frontend; returns net, delta, weight (, eta, upmask NHWC)."""
-        import numpy as np
+        from .corr import coords_grid
+        from .graph import agg_tables
         E, H, W, _ = net.shape
         dev = net.device
-        yy, xx = torch.meshgrid(torch.arange(H, device=dev).float(), torch.arange(W, device=dev).float(), indexing="ij")
-        coords0 = torch.stack([xx, yy], -1).contiguous()
+        coords0 = coords_grid(H, W, dev)
         m = motion.float().permute(0, 2, 3, 1)
         coords1 = (coords0[None] + m[..., 0:2]).contiguous()
         target = (coords1 + m[..., 2:4]).contiguous()
-        agg = None
-        if ii is not None:
-            ux, inv = np.unique(ii.cpu().numpy(), return_inverse=True)
-            order = np.argsort(inv, kind="stable").astype(np.int32)
-            ptr = np.zeros(len(ux) + 1, np.int32); np.cumsum(np.bincount(inv, minlength=len(ux)), out=ptr[1:])
-            agg = (torch.as_tensor(ptr, device=dev), torch.as_tensor(order, device=dev), len(ux))
+        agg = None if ii is None else agg_tables(ii.cpu().numpy(), dev)
         out = self(net, inp, corr, coords1, coords0, target=target, agg=agg)
         delta = out[1] - coords1
         if ii is None:

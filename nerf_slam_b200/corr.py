@@ -16,6 +16,12 @@ from . import _lib
 from . import droid_backends as db
 
 
+def coords_grid(ht, wd, device):
+    """pixel coordinates [ht,wd,2] (x, y) fp32: the identity flow (networks/geom/projective_ops.py:14-19)"""
+    y, x = torch.meshgrid(torch.arange(ht, device=device).float(), torch.arange(wd, device=device).float(), indexing="ij")
+    return torch.stack([x, y], dim=-1)
+
+
 def to_nhwc_half(fmap):
     """[..., C, H, W] -> [..., H, W, C] contiguous fp16"""
     return fmap.half().movedim(-3, -1).contiguous()

@@ -30,8 +30,8 @@ import torch.nn.functional as F
 
 from . import _lib
 from . import droid_backends as db
-from .corr import AltCorrBlock, CorrPool
-from .graph import proximity_edges
+from .corr import AltCorrBlock, CorrPool, coords_grid
+from .graph import EdgeList, agg_tables, neighborhood_edges, proximity_edges
 
 
 # ----------------------------------------------------------------------------------------------- helpers
@@ -43,12 +43,6 @@ def _se3_inverse(tq):
     c = torch.cross(u, t, dim=1)
     rt = t + 2.0 * (qi[:, 3:] * c + torch.cross(u, c, dim=1))          # R(qi) t
     return torch.cat([-rt, qi], dim=1).contiguous()
-
-
-def coords_grid(ht, wd, device):
-    """networks/geom/projective_ops.py:14-19 -> [ht,wd,2] (x,y)"""
-    y, x = torch.meshgrid(torch.arange(ht, device=device).float(), torch.arange(wd, device=device).float(), indexing="ij")
-    return torch.stack([x, y], dim=-1)
 
 
 def _host_index(v):
@@ -65,17 +59,10 @@ def _host_mask(m):
     return np.asarray(m, dtype=bool).reshape(-1)
 
 
-def _to_dev(a, device, dtype=torch.long):
-    """host index array -> tensor on `device` (pinned, non-blocking upload on CUDA)"""
-    if torch.device(device).type == "cuda":
-        return _lib.h2d(np.ascontiguousarray(a), device, dtype)
-    return torch.from_numpy(np.ascontiguousarray(a)).to(dtype)
-
-
 def _dev_index(v, device):
     if torch.is_tensor(v) and v.device.type == torch.device(device).type:
         return v.reshape(-1).long()
-    return _to_dev(_host_index(v), device)
+    return _lib.h2d(_host_index(v), device)
 
 
 def _nhwc(t):
@@ -316,13 +303,19 @@ def _make_pool(capacity, ht, wd, device):
 
 class _VolumeStore:
     """`FactorGraph.correlation_volumes` for corr_impl == "volume": a growable slot arena of 4-level pyramids.
-    Callable like the reference's CorrBlock: store(coords [1,E,ht,wd,2]) -> [1,E,196,ht,wd]."""
+    Callable like the reference's CorrBlock: store(coords [1,E,ht,wd,2]) -> [1,E,196,ht,wd].
+    The slot of each active edge is kept by the graph's edge list (`edges`, a graph.EdgeList)."""
 
-    def __init__(self, ht, wd, device, capacity):
+    def __init__(self, ht, wd, device, capacity, edges):
         self.ht, self.wd, self.device = ht, wd, device
         self.pool = _make_pool(capacity, ht, wd, device)
-        self.slots = np.zeros(0, np.int64)       # slot of every active edge, in edge order
-        self._slots_d = None
+        self.edges = edges
+        self._slots_src = self._slots_d = None
+
+    @property
+    def slots(self):
+        """slot of every active edge, in edge order"""
+        return self.edges.slots
 
     def __len__(self):
         return int(self.slots.shape[0])
@@ -333,14 +326,14 @@ class _VolumeStore:
         new = _make_pool(cap, self.ht, self.wd, self.device)
         used = sorted(set(range(old.capacity)) - set(old.free))
         if used and hasattr(old, "levels"):
-            idx = _to_dev(np.asarray(used, np.int64), self.device)
+            idx = _lib.h2d(np.asarray(used, np.int64), self.device)
             for a, b in zip(new.levels, old.levels):
                 a.index_copy_(0, idx, b.index_select(0, idx))
         new.free = [s for s in range(cap - 1, -1, -1) if s not in set(used)]
         self.pool = new
 
     def add(self, fmaps, fi, fj):
-        """fmaps [N,rig,128,h,w] (any strides); fi/fj flat frame indices (host) of the new edges"""
+        """fmaps [N,rig,128,h,w] (any strides); fi/fj flat frame indices (host) of the new edges -> their slots"""
         n = len(fi)
         if n > len(self.pool.free):
             self._grow(n)
@@ -349,19 +342,15 @@ class _VolumeStore:
         frames, inv = np.unique(np.concatenate([fi, fj]), return_inverse=True)
         N, rig = fmaps.shape[:2]
         sel = fmaps.reshape(N * rig, *fmaps.shape[2:]) if fmaps.is_contiguous() else fmaps.flatten(0, 1)
-        f = _nhwc(sel[_to_dev(frames, fmaps.device)].to(self.device)).half()
+        f = _nhwc(sel[_lib.h2d(frames, fmaps.device)].to(self.device)).half()
         self.pool.build(f, inv[:n].tolist(), inv[n:].tolist(), slots.tolist())
-        self.slots = np.concatenate([self.slots, slots])
-        self._slots_d = None
-
-    def keep(self, keep_mask):
-        self.pool.release(self.slots[~keep_mask].tolist())
-        self.slots = self.slots[keep_mask]
-        self._slots_d = None
+        return slots
 
     def slots_dev(self):
-        if self._slots_d is None:
-            self._slots_d = _to_dev(self.slots.astype(np.int32), self.device, torch.int32)
+        # EdgeList replaces its slot array on every change (never writes it in place): upload once per array
+        if self._slots_src is not self.slots:
+            self._slots_src = self.slots
+            self._slots_d = _lib.h2d(self._slots_src, self.device, torch.int32)
         return self._slots_d
 
     def lookup_nhwc(self, coords, out=None):
@@ -385,152 +374,115 @@ class FactorGraph:
         self.ht = ht = video.ht // 8
         self.wd = wd = video.wd // 8
         self.coords0 = coords_grid(ht, wd, device)
-        z = lambda: np.zeros(0, np.int64)
-        self._ii, self._jj, self._age = z(), z(), z()
-        self._ii_inac, self._jj_inac, self._ii_bad, self._jj_bad = z(), z(), z(), z()
+        self.edges = EdgeList(device, ht, wd)
         self.correlation_volumes = None            # _VolumeStore, created by the first add_factors ("volume")
-        self._net = self._inp = None               # [E,ht,wd,C] channels-last
-        e = lambda: torch.zeros(0, ht, wd, 2, device=device, dtype=torch.float32)
-        self._flow, self._conf, self._target_inac, self._weight_inac = e(), e(), e(), e()
         self.damping = 1e-6 * torch.ones_like(video.disps)
         self._dev = None                           # device copies of the edge lists (per edge set)
 
-    # ---- reference-shaped views of the state
+    # ---- reference-shaped views of the edge list
     def _idx_prop(name):
         def get(self):
-            return torch.from_numpy(getattr(self, name))            # shares memory: `graph.age += 1` works in place
+            return torch.from_numpy(getattr(self.edges, name))      # shares memory: `graph.age += 1` works in place
 
         def set_(self, v):
-            setattr(self, name, np.ascontiguousarray(_host_index(v)))
+            setattr(self.edges, name, np.ascontiguousarray(_host_index(v)))
             self._dev = None
         return property(get, set_)
 
-    ii, jj, age = _idx_prop("_ii"), _idx_prop("_jj"), _idx_prop("_age")
-    ii_inac, jj_inac = _idx_prop("_ii_inac"), _idx_prop("_jj_inac")
-    ii_bad, jj_bad = _idx_prop("_ii_bad"), _idx_prop("_jj_bad")
+    ii, jj, age = _idx_prop("ii"), _idx_prop("jj"), _idx_prop("age")
+    ii_inac, jj_inac = _idx_prop("ii_inac"), _idx_prop("jj_inac")
+    ii_bad, jj_bad = _idx_prop("ii_bad"), _idx_prop("jj_bad")
 
     def _edge_prop(name):
         def get(self):
-            return getattr(self, name)[None]                        # [1,E,ht,wd,2]
+            return getattr(self.edges, name)[None]                  # [1,E,ht,wd,2]
 
         def set_(self, v):
-            setattr(self, name, v.reshape(-1, self.ht, self.wd, 2).to(self.device, torch.float32))
+            setattr(self.edges, name, v.reshape(-1, self.ht, self.wd, 2).to(self.device, torch.float32))
         return property(get, set_)
 
-    gru_estimated_flow, gru_estimated_flow_weight = _edge_prop("_flow"), _edge_prop("_conf")
-    target_inac, weight_inac = _edge_prop("_target_inac"), _edge_prop("_weight_inac")
+    gru_estimated_flow, gru_estimated_flow_weight = _edge_prop("flow"), _edge_prop("weight")
+    target_inac, weight_inac = _edge_prop("flow_inac"), _edge_prop("weight_inac")
 
     def _state_prop(name):
         def get(self):
-            t = getattr(self, name)
+            t = getattr(self.edges, name)
             return None if t is None else t.permute(0, 3, 1, 2)[None]     # [1,E,C,ht,wd] view
 
         def set_(self, v):
-            setattr(self, name, None if v is None else _nhwc(v.reshape(-1, *v.shape[-3:])))
+            setattr(self.edges, name, None if v is None else _nhwc(v.reshape(-1, *v.shape[-3:])))
         return property(get, set_)
 
-    gru_hidden_states, gru_contexts_input = _state_prop("_net"), _state_prop("_inp")
+    gru_hidden_states, gru_contexts_input = _state_prop("net"), _state_prop("inp")
     del _idx_prop, _edge_prop, _state_prop
 
     def _edges_dev(self):
         """(ii, jj) on the device + GraphAgg tables, built once per edge set"""
         if self._dev is None:
-            d = types.SimpleNamespace()
-            d.ii, d.jj = _to_dev(self._ii, self.device), _to_dev(self._jj, self.device)
-            d.ux, inv = np.unique(self._ii, return_inverse=True)
-            order = np.argsort(inv, kind="stable").astype(np.int32)
-            ptr = np.zeros(len(d.ux) + 1, np.int32)
-            np.cumsum(np.bincount(inv, minlength=len(d.ux)), out=ptr[1:])
-            d.agg = (_to_dev(ptr, self.device, torch.int32), _to_dev(order, self.device, torch.int32), len(d.ux))
-            d.ux_d = _to_dev(d.ux, self.device)
-            self._dev = d
+            e, dev = self.edges, self.device
+            self._dev = types.SimpleNamespace(ii=_lib.h2d(e.ii, dev), jj=_lib.h2d(e.jj, dev),
+                                              agg=agg_tables(e.ii, dev), ux=_lib.h2d(np.unique(e.ii), dev))
         return self._dev
 
     # ---- edge bookkeeping
-    def _filter_repeated_edges(self, ii, jj):
-        """:43-54 — drop edges that are already active or inactive"""
-        have = np.concatenate([self._ii * 65536 + self._jj, self._ii_inac * 65536 + self._jj_inac])
-        keep = ~np.isin(ii * 65536 + jj, have)
-        return ii[keep], jj[keep]
-
     def print_edges(self):
         """:56-68"""
-        ix = np.argsort(self._ii, kind="stable")
-        w = self._conf.mean(dim=[1, 2, 3]).cpu().numpy()
-        for e in zip(self._ii[ix], self._jj[ix], w[ix]):
-            print(e)
+        e = self.edges
+        ix = np.argsort(e.ii, kind="stable")
+        w = e.weight.mean(dim=[1, 2, 3]).cpu().numpy()
+        for edge in zip(e.ii[ix], e.jj[ix], w[ix]):
+            print(edge)
         print()
 
     def filter_edges(self):
         """:70-77 — retire long-range edges the network has no confidence in"""
-        conf = self._conf.mean(dim=[1, 2, 3]).cpu().numpy()
-        mask = (np.abs(self._ii - self._jj) > 2) & (conf < 0.001)
-        self._ii_bad = np.concatenate([self._ii_bad, self._ii[mask]])
-        self._jj_bad = np.concatenate([self._jj_bad, self._jj[mask]])
+        e = self.edges
+        conf = e.weight.mean(dim=[1, 2, 3]).cpu().numpy()
+        mask = (np.abs(e.ii - e.jj) > 2) & (conf < 0.001)
+        e.ii_bad = np.concatenate([e.ii_bad, e.ii[mask]])
+        e.jj_bad = np.concatenate([e.jj_bad, e.jj[mask]])
         self.rm_factors(mask, store=False)
 
     def clear_edges(self):
         """:79-82"""
-        self.rm_factors(self._ii >= 0)
-        self._net = self._inp = None
+        self.rm_factors(self.edges.ii >= 0)
+        self.edges.net = self.edges.inp = None
 
     @torch.no_grad()
     def add_factors(self, ii, jj, remove=False):
         """:85-139"""
-        ii, jj = _host_index(ii), _host_index(jj)
-        ii, jj = self._filter_repeated_edges(ii, jj)
-        if ii.shape[0] == 0:
+        ii, jj = self.edges.filter_repeated(_host_index(ii), _host_index(jj))
+        new = ii.shape[0]
+        if new == 0:
             return
-        old, new = self._ii.shape[0], ii.shape[0]
-        if self.max_factors > 0 and old + new > self.max_factors and self.correlation_volumes is not None and remove:
-            # `ix` is argsort(age) (ties in index order, as torch's CPU sort yields); the mask is then applied
-            # POSITIONALLY to the edges — the reference's own quirk (:107-108), kept
-            ix = np.argsort(self._age, kind="stable")
-            self.rm_factors(ix >= self.max_factors - new, store=True)
-        self._ii = np.concatenate([self._ii, ii]); self._jj = np.concatenate([self._jj, jj])
-        self._age = np.concatenate([self._age, np.zeros(new, np.int64)])
-        self._dev = None
+        if remove and self.correlation_volumes is not None:
+            self.rm_factors(self.edges.retire_mask(new, self.max_factors), store=True)
         video = self.video
+        slots = np.zeros(new, np.int64)
         if self.corr_impl == "volume":
             rig = video.fmaps.shape[1]
             if self.correlation_volumes is None:
                 cap = 2 * self.max_factors if self.max_factors > 0 else max(64, 2 * new)
-                self.correlation_volumes = _VolumeStore(self.ht, self.wd, self.device, max(cap, new))
-            self.correlation_volumes.add(video.fmaps, ii * rig, jj * rig + (ii == jj))
-        vi = _to_dev(ii, video.nets.device)
+                self.correlation_volumes = _VolumeStore(self.ht, self.wd, self.device, max(cap, new), self.edges)
+            slots = self.correlation_volumes.add(video.fmaps, ii * rig, jj * rig + (ii == jj))
+        vi = _lib.h2d(ii, video.nets.device)
         net = _nhwc(video.nets[vi]).to(self.device)
         inp = _nhwc(video.inps[vi]).to(self.device)
-        self._net = net if self._net is None else torch.cat([self._net, net], 0)
-        self._inp = inp if self._inp is None else torch.cat([self._inp, inp], 0)
         target, _ = video.reproject(ii, jj)                              # flow initialised with the reprojection
         target = target.reshape(new, self.ht, self.wd, 2).to(self.device, torch.float32)
-        self._flow = torch.cat([self._flow, target], 0)
-        self._conf = torch.cat([self._conf, torch.zeros_like(target)], 0)
+        self.edges.append(ii, jj, slots, net, target, torch.zeros_like(target), inp)
+        self._dev = None
 
     @torch.no_grad()
     def rm_factors(self, mask, store=False):
         """:144-167"""
         mask = _host_mask(mask)
-        if mask.shape[0] == 0 or not mask.any():
+        if not mask.any():
             return
-        keep = ~mask
-        kd = _to_dev(np.nonzero(keep)[0], self.device)
-        if store:
-            rd = _to_dev(np.nonzero(mask)[0], self.device)
-            self._ii_inac = np.concatenate([self._ii_inac, self._ii[mask]])
-            self._jj_inac = np.concatenate([self._jj_inac, self._jj[mask]])
-            self._target_inac = torch.cat([self._target_inac, self._flow.index_select(0, rd)], 0)
-            self._weight_inac = torch.cat([self._weight_inac, self._conf.index_select(0, rd)], 0)
-        self._ii, self._jj, self._age = self._ii[keep], self._jj[keep], self._age[keep]
+        slots = self.edges.remove(mask, store)
         self._dev = None
         if self.corr_impl == "volume" and self.correlation_volumes is not None:
-            self.correlation_volumes.keep(keep)
-        if self._net is not None:
-            self._net = self._net.index_select(0, kd)
-        if self._inp is not None:
-            self._inp = self._inp.index_select(0, kd)
-        self._flow = self._flow.index_select(0, kd)
-        self._conf = self._conf.index_select(0, kd)
+            self.correlation_volumes.pool.release(slots.tolist())
 
     @torch.no_grad()
     def rm_keyframe(self, ix):
@@ -540,32 +492,23 @@ class FactorGraph:
             for name in ("images", "poses", "disps", "disps_sens", "intrinsics", "nets", "inps", "fmaps"):
                 buf = getattr(video, name)
                 buf[ix] = buf[ix + 1]
-        m = (self._ii_inac == ix) | (self._jj_inac == ix)
-        self._ii_inac[self._ii_inac >= ix] -= 1
-        self._jj_inac[self._jj_inac >= ix] -= 1
-        if m.any():
-            kd = _to_dev(np.nonzero(~m)[0], self.device)
-            self._ii_inac, self._jj_inac = self._ii_inac[~m], self._jj_inac[~m]
-            self._target_inac = self._target_inac.index_select(0, kd)
-            self._weight_inac = self._weight_inac.index_select(0, kd)
-        m = (self._ii == ix) | (self._jj == ix)
-        self._ii[self._ii >= ix] -= 1
-        self._jj[self._jj >= ix] -= 1
+        m = self.edges.remove_keyframe(ix)
         self._dev = None
         self.rm_factors(m, store=False)
 
     # ---- the update operator + BA
     def _ba_inputs(self, t0, use_inactive, EP):
         """:229-244 -> (ii, jj, target [E,2,ht,wd], weight [E,2,ht,wd], damping [K,ht,wd])"""
+        e = self.edges
         if use_inactive:
-            m = (self._ii_inac >= t0 - 3) & (self._jj_inac >= t0 - 3)
-            md = _to_dev(np.nonzero(m)[0], self.device)
-            ii = np.concatenate([self._ii_inac[m], self._ii]); jj = np.concatenate([self._jj_inac[m], self._jj])
-            flow = torch.cat([self._target_inac.index_select(0, md), self._flow], 0)
-            conf = torch.cat([self._weight_inac.index_select(0, md), self._conf], 0)
+            m = (e.ii_inac >= t0 - 3) & (e.jj_inac >= t0 - 3)
+            md = _lib.h2d(np.nonzero(m)[0], self.device)
+            ii = np.concatenate([e.ii_inac[m], e.ii]); jj = np.concatenate([e.jj_inac[m], e.jj])
+            flow = torch.cat([e.flow_inac.index_select(0, md), e.flow], 0)
+            conf = torch.cat([e.weight_inac.index_select(0, md), e.weight], 0)
         else:
-            ii, jj, flow, conf = self._ii, self._jj, self._flow, self._conf
-        damping = .2 * self.damping[_to_dev(np.unique(ii), self.device)].contiguous() + EP
+            ii, jj, flow, conf = e.ii, e.jj, e.flow, e.weight
+        damping = .2 * self.damping[_lib.h2d(np.unique(ii), self.device)].contiguous() + EP
         return ii, jj, flow.permute(0, 3, 1, 2).contiguous(), conf.permute(0, 3, 1, 2).contiguous(), damping
 
     def _operator(self, net, inp, corr_fn, coords1, flow, ii_host, agg=None):
@@ -575,17 +518,13 @@ class FactorGraph:
         fused = getattr(self.update_net, "fused", None)
         if fused is not None:
             if agg is None:
-                ux, inv = np.unique(ii_host, return_inverse=True)
-                order = np.argsort(inv, kind="stable").astype(np.int32)
-                ptr = np.zeros(len(ux) + 1, np.int32)
-                np.cumsum(np.bincount(inv, minlength=len(ux)), out=ptr[1:])
-                agg = (_to_dev(ptr, self.device, torch.int32), _to_dev(order, self.device, torch.int32), len(ux))
+                agg = agg_tables(ii_host, self.device)
             out = fused(net, inp, corr_fn(coords1, True), coords1.contiguous(), self.coords0, target=flow.contiguous(), agg=agg)
             eta = 0.01 * F.softplus(out[3][..., 0].float())
             return out[0], out[1], out[2], eta, out[4].permute(0, 3, 1, 2)
         # any callable with UpdateModule.forward's convention (networks/droid_net.py:118-150)
         motion = torch.cat([coords1 - self.coords0, flow - coords1], dim=-1).permute(0, 3, 1, 2).clamp(-64.0, 64.0)
-        ii_t = _to_dev(ii_host, self.device)
+        ii_t = _lib.h2d(ii_host, self.device)
         net2, delta, weight, eta, upmask = self.update_net(net.permute(0, 3, 1, 2)[None], inp.permute(0, 3, 1, 2)[None],
                                                            corr_fn(coords1, False), motion[None], ii_t, ii_t)
         return _nhwc(net2[0]), coords1 + delta[0].float(), weight[0].float(), eta[0].float(), upmask[0]
@@ -593,41 +532,40 @@ class FactorGraph:
     @torch.no_grad()
     def update(self, t0=None, t1=None, itrs=2, use_inactive=False, EP=1e-7, motion_only=False):
         """:202-255 — reproject, correlation lookup, update operator, dense BA"""
-        video, d = self.video, self._edges_dev()
+        video, e, d = self.video, self.edges, self._edges_dev()
         coords1, _ = video.reproject(d.ii, d.jj)
         coords1 = coords1.reshape(-1, self.ht, self.wd, 2)
         store = self.correlation_volumes
         corr_fn = lambda c, nhwc: store.lookup_nhwc(c) if nhwc else store(c[None])
-        net, flow, conf, eta, upmask = self._operator(self._net, self._inp, corr_fn, coords1, self._flow, self._ii, d.agg)
-        self._net, self._flow, self._conf = net, flow, conf
+        e.net, e.flow, e.weight, eta, upmask = self._operator(e.net, e.inp, corr_fn, coords1, e.flow, e.ii, d.agg)
         if t0 is None:
-            t0 = max(1, int(self._ii.min()) + 1)
-        self.damping[d.ux_d] = eta
+            t0 = max(1, int(e.ii.min()) + 1)
+        self.damping[d.ux] = eta
         ii, jj, target, weight, damping = self._ba_inputs(t0, use_inactive, EP)
         video.ba(target, weight, damping, ii, jj, t0, t1, itrs=itrs, lm=1e-4, ep=0.1, motion_only=motion_only)
         if self.upsample:
-            video.upsample(d.ux_d, upmask)
-        self._age += 1
+            video.upsample(d.ux, upmask)
+        e.age += 1
 
     @torch.no_grad()
     def update_lowmem(self, t0=None, t1=None, itrs=2, use_inactive=False, EP=1e-7, steps=8):
         """:259-303 — global BA: on-the-fly correlation (alt-corr), edges in chunks of 8 source frames"""
-        video = self.video
+        video, e = self.video, self.edges
         t = video.counter.value
         num, rig, ch, ht, wd = video.fmaps.shape
         corr_op = AltCorrBlock(video.fmaps.reshape(1, num * rig, ch, ht, wd))
         from .conv import CORR_PAD
         for step in range(steps):
-            coords1, _ = video.reproject(self._ii, self._jj)
+            coords1, _ = video.reproject(e.ii, e.jj)
             coords1 = coords1.reshape(-1, self.ht, self.wd, 2)
             s = 8
-            for i in range(0, int(self._jj.max()) + 1, s):
-                v = (self._ii >= i) & (self._ii < i + s)
+            for i in range(0, int(e.jj.max()) + 1, s):
+                v = (e.ii >= i) & (e.ii < i + s)
                 if not v.any():
                     continue
-                vd = _to_dev(np.nonzero(v)[0], self.device)
-                iis, jjs = self._ii[v], self._jj[v]
-                fi = _to_dev(rig * iis, self.device); fj = _to_dev(rig * jjs + (iis == jjs), self.device)
+                vd = _lib.h2d(np.nonzero(v)[0], self.device)
+                iis, jjs = e.ii[v], e.jj[v]
+                fi = _lib.h2d(rig * iis, self.device); fj = _lib.h2d(rig * jjs + (iis == jjs), self.device)
                 c1 = coords1.index_select(0, vd)
 
                 def corr_fn(c, nhwc, fi=fi, fj=fj):
@@ -635,28 +573,23 @@ class FactorGraph:
                     if not nhwc:
                         return corr
                     return F.pad(corr[0].permute(0, 2, 3, 1), (0, CORR_PAD - corr.shape[2])).half().contiguous()
-                inp = _nhwc(video.inps[_to_dev(iis, video.inps.device)]).to(self.device)
-                net, flow, conf, eta, upmask = self._operator(self._net.index_select(0, vd), inp, corr_fn, c1,
-                                                              self._flow.index_select(0, vd), iis)
-                self._net.index_copy_(0, vd, net)
-                self._flow.index_copy_(0, vd, flow)
-                self._conf.index_copy_(0, vd, conf)
-                self.damping[_to_dev(np.unique(iis), self.device)] = eta
-            damping = .2 * self.damping[_to_dev(np.unique(self._ii), self.device)].contiguous() + EP
-            target = self._flow.permute(0, 3, 1, 2).contiguous()
-            weight = self._conf.permute(0, 3, 1, 2).contiguous()
-            video.ba(target, weight, damping, self._ii, self._jj, 1, t, itrs=itrs, lm=1e-5, ep=1e-2, motion_only=False)
+                inp = _nhwc(video.inps[_lib.h2d(iis, video.inps.device)]).to(self.device)
+                net, flow, conf, eta, upmask = self._operator(e.net.index_select(0, vd), inp, corr_fn, c1,
+                                                              e.flow.index_select(0, vd), iis)
+                e.net.index_copy_(0, vd, net)
+                e.flow.index_copy_(0, vd, flow)
+                e.weight.index_copy_(0, vd, conf)
+                self.damping[_lib.h2d(np.unique(iis), self.device)] = eta
+            damping = .2 * self.damping[_lib.h2d(np.unique(e.ii), self.device)].contiguous() + EP
+            target = e.flow.permute(0, 3, 1, 2).contiguous()
+            weight = e.weight.permute(0, 3, 1, 2).contiguous()
+            video.ba(target, weight, damping, e.ii, e.jj, 1, t, itrs=itrs, lm=1e-5, ep=1e-2, motion_only=False)
             video.dirty[:t] = True
 
     # ---- edge creation
     def add_neighborhood_factors(self, t0, t1, r=3):
         """:305-320 — edges between frames of [t0,t1) whose index distance is in (c, r]"""
-        ii, jj = np.meshgrid(np.arange(t0, t1), np.arange(t0, t1), indexing="ij")
-        ii, jj = ii.reshape(-1), jj.reshape(-1)
-        c = 1 if self.video.stereo else 0
-        d = np.abs(ii - jj)
-        keep = (d > c) & (d <= r)
-        self.add_factors(ii[keep], jj[keep])
+        self.add_factors(*neighborhood_edges(t0, t1, r, self.video.stereo))
 
     def add_proximity_factors(self, t0=0, t1=0, rad=2, nms=2, beta=0.25, thresh=16.0, remove=False):
         """:323-387 — edges to frames that are close in mean-flow distance, with non-maximum suppression around
@@ -667,9 +600,7 @@ class FactorGraph:
         ii, jj = ii.reshape(-1), jj.reshape(-1)
         d = self.video.distance(ii, jj, beta=beta)
         d = d.detach().float().cpu().numpy().copy()
-        ii1 = np.concatenate([self._ii, self._ii_bad, self._ii_inac])
-        jj1 = np.concatenate([self._jj, self._jj_bad, self._jj_inac])
-        es = proximity_edges(d, ii, jj, ii1, jj1, t0, t1, t, rad, nms, thresh, self.max_factors, self.video.stereo)
+        es = proximity_edges(d, ii, jj, *self.edges.known(), t0, t1, t, rad, nms, thresh, self.max_factors, self.video.stereo)
         if es.shape[0] == 0:
             return
         self.add_factors(es[:, 0], es[:, 1], remove)

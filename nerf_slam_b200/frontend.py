@@ -25,8 +25,8 @@ import torch
 
 from . import droid_backends as db
 from . import _lib
-from .corr import CorrPool, AltCorrBlock
-from .graph import proximity_edges
+from .corr import CorrPool, AltCorrBlock, coords_grid
+from .graph import EdgeList, agg_tables, neighborhood_edges, proximity_edges
 from .conv import CORR_PAD as CORR_PAD_
 from .networks import BasicEncoder, UpdateModule, load_droid_weights
 
@@ -79,12 +79,6 @@ def types_ns(**kw):
     return types.SimpleNamespace(**kw)
 
 
-def coords_grid(ht, wd, device):
-    y, x = torch.meshgrid(torch.arange(ht, device=device).float(), torch.arange(wd, device=device).float(),
-                          indexing="ij")
-    return torch.stack([x, y], dim=-1)
-
-
 class _Timers:
     """optional wall-clock section timers of the HOST thread (NSLAM_TIMERS=1); no device syncs are added"""
 
@@ -117,6 +111,11 @@ class _Section:
         return False
 
 
+def _edge_attr(name):
+    """attribute `name` of the edge list (`self.edges`), readable and assignable on the front end"""
+    return property(lambda self: getattr(self.edges, name), lambda self, v: setattr(self.edges, name, v))
+
+
 class EmptyValues:
     """what the reference's forward() hands to its (no-op) back-end: an EMPTY gtsam.Values / NonlinearFactorGraph
     (visual_frontend.py:248-249).  They must not be None — VioSLAM._frontend stops the pipeline on `x0 is None`
@@ -137,6 +136,14 @@ class EmptyFactorGraph(EmptyValues):
 
 
 class RaftVisualFrontend:
+    # the edge list (graph.EdgeList) under this class' names: host index lists *_h, per-edge state gru_* (the reference's
+    # names; gru_hidden_states is [E,ht,wd,128] fp16 channels-last).  ii / jj / slots_d are their device copies.
+    ii_h, jj_h, age_h, slots_h = _edge_attr("ii"), _edge_attr("jj"), _edge_attr("age"), _edge_attr("slots")
+    ii_inactive_h, jj_inactive_h = _edge_attr("ii_inac"), _edge_attr("jj_inac")
+    ii_bad_h, jj_bad_h = _edge_attr("ii_bad"), _edge_attr("jj_bad")
+    gru_hidden_states, gru_estimated_flow, gru_estimated_flow_weight = _edge_attr("net"), _edge_attr("flow"), _edge_attr("weight")
+    gru_estimated_flow_inactive, gru_estimated_flow_weight_inactive = _edge_attr("flow_inac"), _edge_attr("weight_inac")
+
     def __init__(self, world_T_body_t0, body_T_cam0, args, device="cuda:0"):
         self.args = args
         self.device = device
@@ -215,10 +222,6 @@ class RaftVisualFrontend:
         self.use_cuda_graphs = bool(getattr(args, "cuda_graphs", True))
         self._static = None
         self._img_static = None
-        # update(): replaying a captured graph saves host time per call but costs a re-capture (~2 ms of host
-        # time with an idle stream) whenever the edge set changes, i.e. once per keyframe.  With the operator as
-        # one C call (use_op_step) the eager path issues ~10 host calls per update and is the default.
-        self.use_update_graphs = self.use_cuda_graphs and bool(getattr(args, "update_graphs", False))
         # the update operator as one C call per update() (csrc/update_step.cu) instead of ~45 ctypes/torch calls
         self.use_op_step = bool(getattr(args, "op_step", True))
         self._graph_pool = torch.cuda.graph_pool_handle() if self.use_cuda_graphs else None
@@ -293,17 +296,8 @@ class RaftVisualFrontend:
         self.viz_idx = np.zeros(B, dtype=bool)          # host-side dirty flags (a device mask would need a sync to read)
 
     def _reset_graph(self):
-        dev, ht, wd = self.device, self.ht, self.wd
-        self.ii_h = np.zeros(0, np.int64); self.jj_h = np.zeros(0, np.int64); self.age_h = np.zeros(0, np.int64)
-        self.slots_h = np.zeros(0, np.int64)
-        self.ii = torch.zeros(0, dtype=torch.long, device=dev); self.jj = torch.zeros(0, dtype=torch.long, device=dev)
-        self.ii_inactive_h = np.zeros(0, np.int64); self.jj_inactive_h = np.zeros(0, np.int64)
-        self.ii_bad_h = np.zeros(0, np.int64); self.jj_bad_h = np.zeros(0, np.int64)
-        self.gru_hidden_states = None          # [E,ht,wd,128] fp16 (NHWC)
-        self.gru_estimated_flow = torch.zeros(0, ht, wd, 2, device=dev)
-        self.gru_estimated_flow_weight = torch.zeros(0, ht, wd, 2, device=dev)
-        self.gru_estimated_flow_inactive = torch.zeros(0, ht, wd, 2, device=dev)
-        self.gru_estimated_flow_weight_inactive = torch.zeros(0, ht, wd, 2, device=dev)
+        self.edges = EdgeList(self.device, self.ht, self.wd)
+        self._sync_edges()
         self.damping = 1e-6 * torch.ones_like(self.cam0_idepths)
         if hasattr(self, "corr_pool"):
             self.corr_pool.free = list(range(self.corr_pool.capacity - 1, -1, -1))
@@ -338,21 +332,12 @@ class RaftVisualFrontend:
         c = self.context_tc(imgs_norm[0]).permute(0, 2, 3, 1)
         return torch.tanh(c[..., :128]), torch.relu(c[..., 128:])
 
-    @staticmethod
-    def _agg_tables(ii_host, device):
-        """CSR of the edges per source keyframe for GraphAgg (host-built: no device sync)"""
-        ux, inv = np.unique(np.asarray(ii_host), return_inverse=True)
-        order = np.argsort(inv, kind="stable").astype(np.int32)
-        ptr = np.zeros(len(ux) + 1, np.int32)
-        np.cumsum(np.bincount(inv, minlength=len(ux)), out=ptr[1:])
-        return (_lib.h2d(ptr, device), _lib.h2d(order, device), len(ux))
-
     def _run_update_net(self, net, inp, corr_nhwc, coords1, target, ii_host=None):
         """update operator on NHWC tensors: net/inp [E,ht,wd,128], corr [E,ht,wd,CORR_PAD], coords1/target
         [E,ht,wd,2] (target None -> zero residual) -> net' [E,ht,wd,128], delta/weight [E,ht,wd,2] fp32
         (, eta [K,ht,wd], upmask NHWC [K,ht,wd,576]) — the reference's UpdateModule return convention
         (droid_net.py:118-150).  ii_host: numpy source indices of the edges (enables GraphAgg)."""
-        agg = None if ii_host is None else self._agg_tables(ii_host, self.device)
+        agg = None if ii_host is None else agg_tables(ii_host, self.device)
         out = self.update_tc(net, inp, corr_nhwc, coords1.contiguous(), self.coords0, target=target, agg=agg)
         delta = out[1] - coords1
         if ii_host is None:
@@ -516,13 +501,8 @@ class RaftVisualFrontend:
 
     # ------------------------------------------------------------------ graph management (A18)
     def add_neighborhood_factors(self, kf0, kf1, radius=3):
-        """visual_frontend.py:690-708"""
-        ii, jj = np.meshgrid(np.arange(kf0, kf1 + 1), np.arange(kf0, kf1 + 1), indexing="ij")
-        ii, jj = ii.reshape(-1), jj.reshape(-1)
-        c = 1 if self.stereo else 0
-        d = np.abs(ii - jj)
-        keep = (d > c) & (d <= radius)
-        self.add_factors(ii[keep], jj[keep])
+        """visual_frontend.py:690-708 (keyframes kf0..kf1 inclusive)"""
+        self.add_factors(*neighborhood_edges(kf0, kf1 + 1, radius, self.stereo))
 
     def distance(self, ii, jj, beta=0.3, bidirectional=True):
         """visual_frontend.py:778-799"""
@@ -546,10 +526,8 @@ class RaftVisualFrontend:
             d = self._take_prefetched_distances(kf0, kf1, t, beta)
             if d is None:
                 d = self.distance(ii, jj, beta=beta).cpu().numpy().copy()
-        ii1 = np.concatenate([self.ii_h, self.ii_bad_h, self.ii_inactive_h])
-        jj1 = np.concatenate([self.jj_h, self.jj_bad_h, self.jj_inactive_h])
         with self.timers.section("prox.selection (host)"):
-            es = proximity_edges(d, ii, jj, ii1, jj1, kf0, kf1, t, rad, nms, thresh, self.max_factors, self.stereo)
+            es = proximity_edges(d, ii, jj, *self.edges.known(), kf0, kf1, t, rad, nms, thresh, self.max_factors, self.stereo)
         if es.shape[0] == 0:
             return
         with self.timers.section("prox.add_factors"):
@@ -587,23 +565,15 @@ class RaftVisualFrontend:
         pf[3].synchronize()
         return self._prox_host[:pf[2]].numpy().copy()
 
-    def _filter_repeated_edges(self, ii, jj):
-        """visual_frontend.py:896-907: drop candidates that are already active or stored as inactive (duplicates INSIDE
-        the candidate list are kept, as in the reference); membership on (i, j) packed into one integer"""
-        have = np.concatenate([self.ii_h * 65536 + self.jj_h, self.ii_inactive_h * 65536 + self.jj_inactive_h])
-        keep = ~np.isin(ii * 65536 + jj, have)
-        return ii[keep], jj[keep]
-
     def add_factors(self, ii, jj, remove=False):
         """visual_frontend.py:807-862"""
         ii = np.asarray(ii, np.int64).reshape(-1); jj = np.asarray(jj, np.int64).reshape(-1)
-        ii, jj = self._filter_repeated_edges(ii, jj)
-        if ii.shape[0] == 0:
+        ii, jj = self.edges.filter_repeated(ii, jj)
+        new = ii.shape[0]
+        if new == 0:
             return
-        old, new = self.ii_h.shape[0], ii.shape[0]
-        if self.max_factors > 0 and old + new > self.max_factors and self.gru_hidden_states is not None and remove:
-            ix = np.arange(len(self.age_h))[np.argsort(self.age_h, kind="stable")]
-            self.rm_factors(ix >= (self.max_factors - new), store=True)
+        if remove and self.gru_hidden_states is not None:
+            self.rm_factors(self.edges.retire_mask(new, self.max_factors), store=True)
         slots = np.zeros(new, np.int64)
         if self.corr_impl == "volume":
             slots = np.asarray(self.corr_pool.alloc(new), np.int64)
@@ -612,43 +582,20 @@ class RaftVisualFrontend:
             fj = (jj * cams + (ii == jj)).tolist()
             fm = self.features_imgs.view(self.buffer * cams, self.ht, self.wd, 128)
             self.corr_pool.build(fm, fi, fj, slots.tolist())
-        self.ii_h = np.concatenate([self.ii_h, ii]); self.jj_h = np.concatenate([self.jj_h, jj])
-        self.age_h = np.concatenate([self.age_h, np.zeros(new, np.int64)])
-        self.slots_h = np.concatenate([self.slots_h, slots])
-        self._sync_edges()
-        iid = _lib.h2d(ii, self.device)
-        hid = self.contexts_imgs[iid, 0]
-        self.gru_hidden_states = hid if self.gru_hidden_states is None else torch.cat([self.gru_hidden_states, hid], 0)
+        hid = self.contexts_imgs[_lib.h2d(ii, self.device), 0]
         target, _ = self.reproject(ii, jj)
-        self.gru_estimated_flow = torch.cat([self.gru_estimated_flow, target], 0)
-        self.gru_estimated_flow_weight = torch.cat([self.gru_estimated_flow_weight, torch.zeros_like(target)], 0)
+        self.edges.append(ii, jj, slots, hid, target, torch.zeros_like(target))
+        self._sync_edges()
 
     def rm_factors(self, mask, store=False):
         """visual_frontend.py:868-892; mask: host bool array over the active edges"""
         mask = np.asarray(mask, dtype=bool)
-        if mask.shape[0] == 0:
-            return
-        # integer index tensors built on the host: boolean-mask indexing would sync the device (nonzero)
         if not mask.any():
             return
-        rm_d = _lib.h2d(np.nonzero(mask)[0], self.device)
-        if store:
-            self.ii_inactive_h = np.concatenate([self.ii_inactive_h, self.ii_h[mask]])
-            self.jj_inactive_h = np.concatenate([self.jj_inactive_h, self.jj_h[mask]])
-            self.gru_estimated_flow_inactive = torch.cat([self.gru_estimated_flow_inactive,
-                                                          self.gru_estimated_flow.index_select(0, rm_d)], 0)
-            self.gru_estimated_flow_weight_inactive = torch.cat(
-                [self.gru_estimated_flow_weight_inactive, self.gru_estimated_flow_weight.index_select(0, rm_d)], 0)
+        slots = self.edges.remove(mask, store)
         if self.corr_impl == "volume":
-            self.corr_pool.release(self.slots_h[mask].tolist())
-        keep = ~mask
-        self.ii_h, self.jj_h, self.age_h, self.slots_h = self.ii_h[keep], self.jj_h[keep], self.age_h[keep], self.slots_h[keep]
+            self.corr_pool.release(slots.tolist())
         self._sync_edges()
-        kd = _lib.h2d(np.nonzero(keep)[0], self.device)
-        if self.gru_hidden_states is not None:
-            self.gru_hidden_states = self.gru_hidden_states.index_select(0, kd)
-        self.gru_estimated_flow = self.gru_estimated_flow.index_select(0, kd)
-        self.gru_estimated_flow_weight = self.gru_estimated_flow_weight.index_select(0, kd)
 
     def rm_keyframe(self, kf):
         """visual_frontend.py:530-574"""
@@ -658,17 +605,7 @@ class RaftVisualFrontend:
                     self.cam0_depths_cov, self.cam0_idepths_sensed, self.cam0_intrinsics, self.features_imgs,
                     self.contexts_imgs, self.cst_contexts_imgs):
             buf[kf] = buf[kf + 1]
-        m = (self.ii_inactive_h == kf) | (self.jj_inactive_h == kf)
-        self.ii_inactive_h[self.ii_inactive_h >= kf] -= 1
-        self.jj_inactive_h[self.jj_inactive_h >= kf] -= 1
-        if m.any():
-            md = _lib.h2d(np.nonzero(~m)[0], self.device)
-            self.ii_inactive_h, self.jj_inactive_h = self.ii_inactive_h[~m], self.jj_inactive_h[~m]
-            self.gru_estimated_flow_inactive = self.gru_estimated_flow_inactive.index_select(0, md)
-            self.gru_estimated_flow_weight_inactive = self.gru_estimated_flow_weight_inactive.index_select(0, md)
-        m = (self.ii_h == kf) | (self.jj_h == kf)
-        self.ii_h[self.ii_h >= kf] -= 1
-        self.jj_h[self.jj_h >= kf] -= 1
+        m = self.edges.remove_keyframe(kf)
         if m.any():
             self.rm_factors(m, store=False)
         else:
@@ -742,17 +679,17 @@ class RaftVisualFrontend:
         """Everything of update() that depends only on the EDGE SET (not on the evolving state) is
         computed once here: device index tensors, gathered GRU inputs, the BA window (graph tables,
         buffers) with the stored flows of the inactive edges already in place.  The per-call body
-        (_update_body) then consists of device work on fixed addresses only -> it can be captured in
-        a CUDA graph and replayed for the 4+2 (or 8+8) updates that share the edge set."""
+        (_update_body) then issues only device work on these fixed buffers, for each of the 4+2 (or 8+8)
+        updates that share the edge set."""
         import types
         dev, ht, wd = self.device, self.ht, self.wd
-        st = types.SimpleNamespace(graph=None, calls=0)
+        st = types.SimpleNamespace()
         ii_h, jj_h = self.ii_h, self.jj_h
         kf0 = max(0, int(ii_h.min()))
         st.kf0, st.EP = kf0, EP
         ux, inv = np.unique(ii_h, return_inverse=True)
         st.ux = _lib.h2d(ux, dev); st.ix = _lib.h2d(inv, dev); st.K = len(ux)
-        st.agg = self._agg_tables(ii_h, dev)
+        st.agg = agg_tables(ii_h, dev)
         st.op_ctx = None
         st.inp = self.cst_contexts_imgs[self.ii, 0].contiguous()
         if use_inactive:
@@ -852,31 +789,14 @@ class RaftVisualFrontend:
     def update(self, kf0=None, kf1=None, itrs=2, use_inactive=False, EP=1e-7, motion_only=False):
         """visual_frontend.py:371-470.  The first call after an edge-set change prepares the static part
         (index tables, BA window, operator workspace); every call then issues ~10 host calls (reproject,
-        lookup, nslam_update_op_step, BA Gauss-Newton, covariances, upsample).  With args.update_graphs the
-        device work is instead captured once per edge set and replayed as a CUDA graph."""
+        lookup, nslam_update_op_step, BA Gauss-Newton, covariances, upsample)."""
         st = self._static
         if st is None or st.use_inactive != use_inactive:
             with self.timers.section("update.prepare_static"):
                 st = self._prepare_static(use_inactive, EP)
             st.use_inactive = use_inactive
             self._static = st
-        cc = self.compute_covariances
-        if self.use_update_graphs and st.calls >= 1:
-            if st.graph is None:
-              with self.timers.section("update.graph capture"):
-                g = torch.cuda.CUDAGraph()
-                cs = self._capture_stream
-                cs.wait_stream(torch.cuda.current_stream())
-                with torch.cuda.stream(cs):
-                    g.capture_begin(pool=self._graph_pool)
-                    self._update_body(st, itrs, cc)
-                    g.capture_end()
-                torch.cuda.current_stream().wait_stream(cs)
-                st.graph = g
-            st.graph.replay()
-        else:
-            self._update_body(st, itrs, cc)
-        st.calls += 1
+        self._update_body(st, itrs, self.compute_covariances)
         self._touch_state()
         self.viz_idx[st.kf0:self.kf_idx + 1] = True
         self.age_h += 1

@@ -101,7 +101,7 @@ class RefCudaFrontend(RaftVisualFrontend):
         if self.refcorr is None or self.refdroid is None:
             raise RuntimeError("oracle/_ref/*.so not built (python -m oracle.build_ref in the build container)")
         self.update_tc = self.feature_tc = self.context_tc = None      # library convolutions (cuDNN, fp16)
-        self.use_cuda_graphs = self.use_update_graphs = self.use_op_step = False
+        self.use_cuda_graphs = self.use_op_step = False
         torch.backends.cudnn.benchmark = True
 
     # ---- buffers: the reference's growing correlation pool instead of the slot arena
