@@ -8,7 +8,10 @@ and the dense grid of tsdf_fusion.py update different voxel sets; TsdfFusion sel
 The pool (tsdf, weight, colour: 80 KB per block) starts at `block_count` blocks and doubles when a keyframe's new
 blocks do not fit; every block keeps its pool index, and new blocks are appended in ascending key order, so the pool is
 the same on every run.  Each keyframe costs one small host read (the numbers of touched and new blocks), which sizes
-the growth and the launch.  Read-outs equal the dense read-outs of the volume's dense embedding (`to_dense`)."""
+the growth and the launch.  Read-outs equal the dense read-outs of the volume's dense embedding (`to_dense`).
+tsdf_fusion.DenseVolume, the dense grid, has the same surface."""
+from functools import partial
+
 import numpy as np
 import torch
 
@@ -19,6 +22,16 @@ BLOCK = 16
 
 def _pow2_at_least(n):
     return 1 << max(1, int(n - 1).bit_length())
+
+
+def raycast_outputs(n, H, W, device, normals, depth=None, color=None, weight=None):
+    """depth [n,H,W], colour [n,H,W,3], weight [n,H,W] and normal [n,H,W,3] (None without `normals`): the caller's
+    tensors where given (the kernels write them through raw pointers, hence the check), else new ones"""
+    def out(t, *ch):
+        if t is not None and (t.shape != (n, H, W, *ch) or t.dtype != torch.float32 or not t.is_contiguous()):
+            raise ValueError(f"ray-cast output {tuple(t.shape)} {t.dtype}: wants a contiguous fp32 {(n, H, W, *ch)}")
+        return torch.empty(n, H, W, *ch, dtype=torch.float32, device=device) if t is None else t
+    return out(depth), out(color, 3), out(weight), out(None, 3) if normals else None
 
 
 class _CudaKernels:
@@ -147,57 +160,40 @@ class VoxelBlockVolume:
     def build_mesh(self, min_weight):
         """marching cubes over the cubes whose 8 corners have weight > min_weight (>= 0) -> TsdfMesh or None.  Vertices by
         (pool index, local voxel, axis)."""
-        from .tsdf_fusion import TsdfMesh
+        from .tsdf_fusion import marching_cubes
         lib = _lib.load()
         if not min_weight >= 0:
             raise ValueError("min_weight must be >= 0: voxels outside the blocks have weight 0")
         if self.n_blocks == 0:
             return None
-        dev = self.device
-        n_scratch = np.zeros(1, np.int64)
-        _lib.check(lib.nslam_tsdf_blocks_mesh_plan(self.n_blocks, n_scratch.ctypes.data), "tsdf_blocks_mesh_plan")
-        scratch = torch.empty(int(n_scratch[0]), dtype=torch.int32, device=dev)
+        nbr = self._neighbours()
+        head = (_lib.ptr(self.tsdf), _lib.ptr(self.weight))
+        blocks = (_lib.ptr(nbr), _lib.ptr(self._coords), self.n_blocks)
         mw = float(min_weight)
-        with _lib.fixed_stream():
-            nbr = self._neighbours()
-            _lib.check(lib.nslam_tsdf_blocks_mesh_count(_lib.ptr(self.tsdf), _lib.ptr(self.weight), _lib.ptr(nbr),
-                                                        _lib.ptr(self._coords), self.n_blocks, mw, _lib.ptr(scratch),
-                                                        _lib.stream_ptr()), "tsdf_blocks_mesh_count")
-            n_vert, n_tri, n_active = scratch[:3].tolist()
-            if n_tri == 0:
-                return None
-            active = torch.empty(n_active, 4, dtype=torch.int32, device=dev)
-            verts = torch.empty(n_vert, 3, dtype=torch.float32, device=dev)
-            cols = torch.empty(n_vert, 3, dtype=torch.float32, device=dev)
-            nrms = torch.empty(n_vert, 3, dtype=torch.float32, device=dev)
-            tris = torch.empty(n_tri, 3, dtype=torch.int32, device=dev)
-            _lib.check(lib.nslam_tsdf_blocks_mesh_emit(
-                _lib.ptr(self.tsdf), _lib.ptr(self.weight), _lib.ptr(self.color), _lib.ptr(nbr), _lib.ptr(self._coords),
-                self.n_blocks, float(self.voxel_size), mw, _lib.ptr(scratch), n_active, _lib.ptr(active), _lib.ptr(verts),
-                _lib.ptr(cols), _lib.ptr(nrms), _lib.ptr(tris), _lib.stream_ptr()), "tsdf_blocks_mesh_emit")
-        return TsdfMesh(verts, tris, cols, nrms)
+        return marching_cubes("tsdf_blocks_mesh", partial(lib.nslam_tsdf_blocks_mesh_plan, self.n_blocks),
+                              partial(lib.nslam_tsdf_blocks_mesh_count, *head, *blocks, mw),
+                              partial(lib.nslam_tsdf_blocks_mesh_emit, *head, _lib.ptr(self.color), *blocks,
+                                      float(self.voxel_size), mw), self.device)
 
-    def raycast(self, cam_T_world_tq, H, W, intrinsics, min_depth, max_depth, sdf_trunc, min_weight, normals=False):
+    def raycast(self, cam_T_world_tq, H, W, intrinsics, min_depth, max_depth, sdf_trunc, min_weight, normals=False,
+                depth=None, color=None, weight=None):
         """ray-cast the views cam_T_world_tq [n,7] in one launch -> depth [n,H,W] (0 = miss), colour [n,H,W,3] in [0,1],
-        weight [n,H,W] and, with `normals`, unit normals [n,H,W,3] (else None)"""
+        weight [n,H,W] and, with `normals`, unit normals [n,H,W,3] (else None).  `depth`, `color` and `weight` may be given
+        as outputs."""
         if not min_weight >= 0:
             raise ValueError("min_weight must be >= 0: voxels outside the blocks have weight 0")
-        dev = self.device
-        poses = cam_T_world_tq.to(dev, torch.float32).contiguous()
+        poses = cam_T_world_tq.to(self.device, torch.float32).contiguous()
         n = poses.shape[0]
-        depth = torch.empty(n, H, W, dtype=torch.float32, device=dev)
-        color = torch.empty(n, H, W, 3, dtype=torch.float32, device=dev)
-        weight = torch.empty(n, H, W, dtype=torch.float32, device=dev)
-        normal = torch.empty(n, H, W, 3, dtype=torch.float32, device=dev) if normals else None
+        out = raycast_outputs(n, H, W, self.device, normals, depth, color, weight)
         intr = np.ascontiguousarray(np.asarray(intrinsics, np.float32))
         with _lib.fixed_stream():
             nbr = self._neighbours()
             _lib.check(_lib.load().nslam_tsdf_blocks_raycast(
                 _lib.ptr(self.tsdf), _lib.ptr(self.weight), _lib.ptr(self.color), _lib.ptr(nbr), _lib.ptr(self._hkeys),
                 _lib.ptr(self._hvals), self._hkeys.numel(), float(self.voxel_size), _lib.ptr(poses), n, H, W, intr.ctypes.data,
-                float(min_depth), float(max_depth), float(sdf_trunc), float(min_weight), _lib.ptr(depth), _lib.ptr(color),
-                _lib.ptr(weight), _lib.ptr(normal), _lib.stream_ptr()), "tsdf_blocks_raycast")
-        return depth, color, weight, normal
+                float(min_depth), float(max_depth), float(sdf_trunc), float(min_weight), *[_lib.ptr(t) for t in out],
+                _lib.stream_ptr()), "tsdf_blocks_raycast")
+        return out
 
     def to_dense(self, margin_blocks=1):
         """dense embedding of the volume (0 outside its blocks), for small volumes and export: tsdf, weight [nz,ny,nx],

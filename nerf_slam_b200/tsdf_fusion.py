@@ -15,24 +15,26 @@ row of `results.csv` (:319-484).  One deliberate deviation there: the reference 
 image / 255 (:406, :459-461); here both sides are on [0, 1], as in its own `sum_colors` path (:413-415).
 
 Differences by design: Open3D's hashed VoxelBlockGrid driven from Python (~40 tensor ops and four device
-synchronisations per keyframe, :185-302) becomes one kernel launch per keyframe on a DENSE grid (csrc/tsdf.cu) —
-the reference's own extent "6 m / 512 voxels" is 2.7 GB at 20 B per voxel on an 80 GB part; poses, depths, weights and
-masks are consumed where the SLAM packet holds them (device tensors; the reference converts each frame to three Open3D
-images and copies the poses to the host).
+synchronisations per keyframe, :185-302) becomes one kernel launch per keyframe on a DENSE grid (DenseVolume,
+csrc/tsdf.cu) — the reference's own extent "6 m / 512 voxels" is 2.7 GB at 20 B per voxel on an 80 GB part; poses,
+depths, weights and masks are consumed where the SLAM packet holds them (device tensors; the reference converts each
+frame to three Open3D images and copies the poses to the host).
 
-`args.tsdf_volume = "blocks"` (default "dense") selects the sparse voxel-block volume of tsdf_blocks.py instead: unbounded,
-16^3 blocks allocated where the depth maps reach (`args.tsdf_block_count` to start with, default 5000, the reference's
-block_count), only the voxels of the blocks a keyframe touches updated, as in the reference — so the two volumes update
-different voxel sets, and the choice is the user's.  Integration, the history rebuild, the reset, both read-outs, the
-GUI packets and `--eval` work on either; `surface_points` is dense-only."""
+TsdfFusion holds one `volume`: a DenseVolume, or with `args.tsdf_volume = "blocks"` (default "dense") the sparse
+voxel-block volume of tsdf_blocks.py: unbounded, 16^3 blocks allocated where the depth maps reach (`args.tsdf_block_count`
+to start with, default 5000, the reference's block_count), only the voxels of the blocks a keyframe touches updated, as in
+the reference — so the two volumes update different voxel sets, and the choice is the user's.  Both have the same surface
+(reset, integrate, build_mesh, raycast, memory_bytes, to_dense), so integration, the history rebuild, the reset, both
+read-outs, the GUI packets and `--eval` work on either; `surface_points` is dense-only."""
 import csv
+from functools import partial
 
 import numpy as np
 import torch
 
 from . import _lib
 from .point_cloud import build_point_cloud as _build_point_cloud, write_binary_ply
-from .tsdf_blocks import VoxelBlockVolume
+from .tsdf_blocks import VoxelBlockVolume, raycast_outputs
 
 
 class TsdfMesh:
@@ -55,6 +57,27 @@ class TsdfMesh:
         write_binary_ply(path, cols, self.triangles.detach().cpu().numpy())
 
 
+def marching_cubes(name, plan, count, emit, device):
+    """the host side of both marching-cubes read-outs: `plan`, `count` and `emit` are nslam_<name>_plan / _count / _emit
+    with the volume's leading arguments bound.  The count passes leave the vertex, triangle and active-voxel totals at the
+    head of the scratch; their one host read sizes the outputs of the emit passes -> TsdfMesh of device tensors, or None
+    when there is no triangle."""
+    n_scratch = np.zeros(1, np.int64)
+    _lib.check(plan(n_scratch.ctypes.data), name + "_plan")
+    scratch = torch.empty(int(n_scratch[0]), dtype=torch.int32, device=device)
+    with _lib.fixed_stream():
+        _lib.check(count(_lib.ptr(scratch), _lib.stream_ptr()), name + "_count")
+        n_vert, n_tri, n_active = scratch[:3].tolist()
+        if n_tri == 0:
+            return None
+        active = torch.empty(n_active, 4, dtype=torch.int32, device=device)
+        verts, cols, nrms = (torch.empty(n_vert, 3, dtype=torch.float32, device=device) for _ in range(3))
+        tris = torch.empty(n_tri, 3, dtype=torch.int32, device=device)
+        _lib.check(emit(_lib.ptr(scratch), n_active, _lib.ptr(active), _lib.ptr(verts), _lib.ptr(cols), _lib.ptr(nrms),
+                        _lib.ptr(tris), _lib.stream_ptr()), name + "_emit")
+    return TsdfMesh(verts, tris, cols, nrms)
+
+
 def mesh_dense(tsdf, weight, color, origin, voxel_size, min_weight):
     """marching cubes (csrc/tsdf_mesh.cu) over a dense [nz,ny,nx] volume whose voxel (i,j,k) sits at origin + voxel_size *
     (i,j,k), over the cubes whose 8 corners have weight > min_weight -> TsdfMesh of device tensors, or None when there is
@@ -62,28 +85,81 @@ def mesh_dense(tsdf, weight, color, origin, voxel_size, min_weight):
     read of the three counts sizes the outputs."""
     lib = _lib.load()
     nz, ny, nx = tsdf.shape
-    dev = tsdf.device
     org = np.ascontiguousarray(np.asarray(origin, np.float32))
-    n_scratch = np.zeros(1, np.int64)
-    _lib.check(lib.nslam_tsdf_mesh_plan(nx, ny, nz, n_scratch.ctypes.data), "tsdf_mesh_plan")
-    scratch = torch.empty(int(n_scratch[0]), dtype=torch.int32, device=dev)
     mw = float(min_weight)
-    with _lib.fixed_stream():
-        _lib.check(lib.nslam_tsdf_mesh_count(_lib.ptr(tsdf), _lib.ptr(weight), nx, ny, nz, mw, _lib.ptr(scratch),
-                                             _lib.stream_ptr()), "tsdf_mesh_count")
-        n_vert, n_tri, n_active = scratch[:3].tolist()
-        if n_tri == 0:
-            return None
-        active = torch.empty(n_active, 4, dtype=torch.int32, device=dev)
-        verts = torch.empty(n_vert, 3, dtype=torch.float32, device=dev)
-        cols = torch.empty(n_vert, 3, dtype=torch.float32, device=dev)
-        nrms = torch.empty(n_vert, 3, dtype=torch.float32, device=dev)
-        tris = torch.empty(n_tri, 3, dtype=torch.int32, device=dev)
-        _lib.check(lib.nslam_tsdf_mesh_emit(
-            _lib.ptr(tsdf), _lib.ptr(weight), _lib.ptr(color), nx, ny, nz, org.ctypes.data, float(voxel_size), mw,
-            _lib.ptr(scratch), n_active, _lib.ptr(active), _lib.ptr(verts), _lib.ptr(cols), _lib.ptr(nrms), _lib.ptr(tris),
-            _lib.stream_ptr()), "tsdf_mesh_emit")
-    return TsdfMesh(verts, tris, cols, nrms)
+    return marching_cubes(
+        "tsdf_mesh", partial(lib.nslam_tsdf_mesh_plan, nx, ny, nz),
+        partial(lib.nslam_tsdf_mesh_count, _lib.ptr(tsdf), _lib.ptr(weight), nx, ny, nz, mw),
+        partial(lib.nslam_tsdf_mesh_emit, _lib.ptr(tsdf), _lib.ptr(weight), _lib.ptr(color), nx, ny, nz, org.ctypes.data,
+                float(voxel_size), mw), tsdf.device)
+
+
+class DenseVolume:
+    """the dense grid, tsdf / weight [nz,ny,nx] fp32 and color [nz,ny,nx,3] fp32 (u8 scale) on `device` with voxel (i,j,k)
+    at origin + voxel_size * (i,j,k); the surface of tsdf_blocks.VoxelBlockVolume.  Built as resolution^3 about `center`."""
+
+    def __init__(self, resolution, center, voxel_size, device="cuda:0"):
+        n = int(resolution)
+        self.device, self.center = device, np.asarray(center, np.float32)
+        self.tsdf = torch.empty(n, n, n, dtype=torch.float32, device=device)
+        self.weight = torch.empty_like(self.tsdf)
+        self.color = torch.empty(n, n, n, 3, dtype=torch.float32, device=device)
+        self.reset(voxel_size)
+
+    @classmethod
+    def from_tensors(cls, tsdf, weight, color, origin, voxel_size):
+        """a volume over existing tensors of any [nz,ny,nx]; without a centre it has no `reset`"""
+        vol = cls.__new__(cls)
+        vol.device, vol.tsdf, vol.weight, vol.color = tsdf.device, tsdf, weight, color
+        vol.origin, vol.voxel_size = np.asarray(origin, np.float32), float(np.float32(voxel_size))
+        return vol
+
+    def reset(self, voxel_size):
+        """empty the grid in place at a new voxel size.  Voxel (i,j,k) sits at origin + voxel_size * (i,j,k) with the lattice
+        passing through the world origin, like the metric voxel coordinates Open3D's VoxelBlockGrid hands out (integer index
+        x voxel_size): same sample points as the reference wherever both volumes have a voxel"""
+        for t in (self.tsdf, self.weight, self.color):
+            t.zero_()
+        vs = np.float32(voxel_size)
+        self.voxel_size = float(vs)
+        self.origin = ((np.round(self.center / vs) - self.tsdf.shape[0] // 2) * vs).astype(np.float32)
+
+    def memory_bytes(self):
+        return sum(t.numel() * t.element_size() for t in (self.tsdf, self.weight, self.color))
+
+    def integrate(self, idepth_up, depth_cov_up, rgb_chw, intrinsics, cam_T_world_tq, max_depth=6.0, sdf_trunc=0.10,
+                  max_weight=20.0, max_depth_sigma=10000.0):
+        """one keyframe, arguments as VoxelBlockVolume.integrate: one nslam_tsdf_integrate launch over the grid"""
+        nz, ny, nx = self.tsdf.shape
+        H, W = rgb_chw.shape[-2:]
+        intr = np.ascontiguousarray(np.asarray(intrinsics, np.float32))
+        _lib.check(_lib.load().nslam_tsdf_integrate(
+            _lib.ptr(self.tsdf), _lib.ptr(self.weight), _lib.ptr(self.color), nx, ny, nz, self.origin.ctypes.data,
+            self.voxel_size, _lib.ptr(idepth_up), _lib.ptr(depth_cov_up), _lib.ptr(rgb_chw), H, W, intr.ctypes.data,
+            _lib.ptr(cam_T_world_tq), float(max_depth), float(sdf_trunc), float(max_weight), float(max_depth_sigma),
+            _lib.stream_ptr()), "tsdf_integrate")
+
+    def build_mesh(self, min_weight):
+        """marching cubes over the cubes whose 8 corners have weight > min_weight -> TsdfMesh or None (mesh_dense)"""
+        return mesh_dense(self.tsdf, self.weight, self.color, self.origin, self.voxel_size, min_weight)
+
+    def raycast(self, cam_T_world_tq, H, W, intrinsics, min_depth, max_depth, sdf_trunc, min_weight, normals=False,
+                depth=None, color=None, weight=None):
+        """as VoxelBlockVolume.raycast: the views cam_T_world_tq [n,7] in one launch -> depth, colour, weight, normal"""
+        poses = cam_T_world_tq.to(self.device, torch.float32).contiguous()
+        n = poses.shape[0]
+        out = raycast_outputs(n, H, W, self.device, normals, depth, color, weight)
+        intr = np.ascontiguousarray(np.asarray(intrinsics, np.float32))
+        nz, ny, nx = self.tsdf.shape
+        _lib.check(_lib.load().nslam_tsdf_raycast(
+            _lib.ptr(self.tsdf), _lib.ptr(self.weight), _lib.ptr(self.color), nx, ny, nz, self.origin.ctypes.data,
+            self.voxel_size, _lib.ptr(poses), n, H, W, intr.ctypes.data, float(min_depth), float(max_depth),
+            float(sdf_trunc), float(min_weight), *[_lib.ptr(t) for t in out], _lib.stream_ptr()), "tsdf_raycast")
+        return out
+
+    def to_dense(self):
+        """tsdf, weight, color and origin: the grid itself"""
+        return self.tsdf, self.weight, self.color, self.origin
 
 
 def depth_l1_cm(rendered_depth, gt_depth):
@@ -120,35 +196,21 @@ class TsdfFusion:
         self.max_weight = 20.0                           # :62
         self.voxel_size = 6.0 / 512                      # :64
         self.sdf_trunc = 0.10                            # :68
-        # dense grid: `grid_resolution` voxels of `voxel_size` centred on `grid_center` (reference: unbounded hashed blocks,
-        # 5000 x 16^3 voxels of capacity; the default here covers its "6 m room")
-        self.grid_resolution = int(getattr(args, "tsdf_resolution", 512))
-        self.grid_center = np.asarray(getattr(args, "tsdf_center", (0.0, 0.0, 0.0)), np.float32)
-        self.volume_type = getattr(args, "tsdf_volume", "dense")
-        if self.volume_type not in ("dense", "blocks"):
-            raise ValueError(f"tsdf_volume must be 'dense' or 'blocks', not {self.volume_type!r}")
-        self.block_count = int(getattr(args, "tsdf_block_count", 5000))
-        self.volume = None                               # the VoxelBlockVolume in "blocks" mode
+        kind = getattr(args, "tsdf_volume", "dense")
+        if kind == "dense":
+            # `tsdf_resolution`^3 voxels centred on `tsdf_center` (reference: unbounded hashed blocks, 5000 x 16^3 voxels of
+            # capacity; the default here covers its "6 m room")
+            self.volume = DenseVolume(int(getattr(args, "tsdf_resolution", 512)), getattr(args, "tsdf_center", (0.0, 0.0, 0.0)),
+                                      self.voxel_size, device)
+        elif kind == "blocks":
+            self.volume = VoxelBlockVolume(self.voxel_size, int(getattr(args, "tsdf_block_count", 5000)), device)
+        else:
+            raise ValueError(f"tsdf_volume must be 'dense' or 'blocks', not {kind!r}")
         self.integrated_frames = 0
-        self.initialize()
 
     def initialize(self):
-        if self.volume_type == "blocks":
-            if self.volume is None:
-                self.volume = VoxelBlockVolume(self.voxel_size, self.block_count, self.device)
-            else:
-                self.volume.reset(self.voxel_size)       # capacity kept
-            return
-        n = self.grid_resolution
-        dev = self.device
-        self.tsdf = torch.zeros(n, n, n, dtype=torch.float32, device=dev)
-        self.weight = torch.zeros(n, n, n, dtype=torch.float32, device=dev)
-        self.color = torch.zeros(n, n, n, 3, dtype=torch.float32, device=dev)
-        # voxel (i, j, k) sits at origin + voxel_size * (i, j, k) with the lattice passing through the world origin, like the
-        # metric voxel coordinates Open3D's VoxelBlockGrid hands out (integer index x voxel_size): same sample points as the
-        # reference wherever both volumes have a voxel
-        vs = np.float32(self.voxel_size)
-        self.origin = ((np.round(self.grid_center / vs) - n // 2) * vs).astype(np.float32)
+        """empty the volume at the current voxel size, in place (the block volume keeps its capacity)"""
+        self.volume.reset(self.voxel_size)
 
     def reset_volume(self):
         """:304-316 — NB the reference re-creates its volume with HALF the voxel size here; kept"""
@@ -270,24 +332,11 @@ class TsdfFusion:
         covs = None if covs is None else covs.to(self.device, torch.float32).contiguous()
         images = packet["cam0_images"].to(self.device).contiguous()
         assert images.dtype == torch.uint8 and images.shape[1] == 3
-        n, _, H, W = images.shape
         intr = np.ascontiguousarray(np.asarray(intrinsics, np.float32))
-        if self.volume is not None:
-            for k in range(n):                           # one host read of the block counts per keyframe
-                self.volume.integrate(idepths[k], covs[k] if covs is not None else None, images[k], intr, poses[k],
-                                      self.max_depth, self.sdf_trunc, self.max_weight, self.max_depth_sigma_thresh)
-            self.integrated_frames += n
-            return
-        lib = _lib.load()
-        n3 = self.grid_resolution
-        with _lib.fixed_stream():
-            for k in range(n):
-                _lib.check(lib.nslam_tsdf_integrate(
-                    _lib.ptr(self.tsdf), _lib.ptr(self.weight), _lib.ptr(self.color), n3, n3, n3, self.origin.ctypes.data,
-                    float(self.voxel_size), _lib.ptr(idepths[k]), _lib.ptr(covs[k]) if covs is not None else None,
-                    _lib.ptr(images[k]), H, W, intr.ctypes.data, _lib.ptr(poses[k]), float(self.max_depth), float(self.sdf_trunc),
-                    float(self.max_weight), float(self.max_depth_sigma_thresh), _lib.stream_ptr()), "tsdf_integrate")
-        self.integrated_frames += n
+        for k in range(images.shape[0]):
+            self.volume.integrate(idepths[k], covs[k] if covs is not None else None, images[k], intr, poses[k],
+                                  self.max_depth, self.sdf_trunc, self.max_weight, self.max_depth_sigma_thresh)
+        self.integrated_frames += images.shape[0]
 
     def rebuild_volume(self):
         """:172-183"""
@@ -301,9 +350,10 @@ class TsdfFusion:
     def surface_points(self, min_weight=0.01, max_points=2_000_000):
         """voxel centres next to a zero crossing of the TSDF along x / y / z with enough weight (a quick look at the
         surface in plain torch; build_mesh is the full read-out) -> [m,3] world points, [m,3] colours.  Dense grid only."""
-        if self.volume is not None:
+        vol = self.volume
+        if not isinstance(vol, DenseVolume):
             raise NotImplementedError("surface_points reads the dense grid; use build_mesh with tsdf_volume='blocks'")
-        t, w = self.tsdf, self.weight
+        t, w = vol.tsdf, vol.weight
         ok = w > min_weight
         m = torch.zeros_like(ok)
         for d in range(3):
@@ -311,15 +361,13 @@ class TsdfFusion:
             cross = ((a * b) < 0) & ok.narrow(d, 0, t.shape[d] - 1) & ok.narrow(d, 1, t.shape[d] - 1)
             m.narrow(d, 0, t.shape[d] - 1).logical_or_(cross)
         idx = m.nonzero()[:max_points]
-        pts = torch.as_tensor(self.origin, device=t.device) + self.voxel_size * idx[:, [2, 1, 0]].float()
-        return pts, self.color[idx[:, 0], idx[:, 1], idx[:, 2]]
+        pts = torch.as_tensor(vol.origin, device=t.device) + vol.voxel_size * idx[:, [2, 1, 0]].float()
+        return pts, vol.color[idx[:, 0], idx[:, 1], idx[:, 2]]
 
     def build_mesh(self, min_weight_for_mesh):
         """:556-573: marching cubes over the cubes whose 8 corners have weight > min_weight_for_mesh -> TsdfMesh, or None
         when there is no triangle.  One host read of the three counts sizes the outputs."""
-        if self.volume is not None:
-            return self.volume.build_mesh(min_weight_for_mesh)
-        return mesh_dense(self.tsdf, self.weight, self.color, self.origin, self.voxel_size, min_weight_for_mesh)
+        return self.volume.build_mesh(min_weight_for_mesh)
 
     def build_point_cloud(self, voxel_size=None, filter_thresh=None, min_views=2):
         """the GUI's build_pcls(None), "rebuild from history" (gui/open3d_gui.py:646-678): every keyframe of the history
@@ -349,7 +397,7 @@ class TsdfFusion:
         if not packet:
             print("Error: asked to render volume, but packet is None.")
             return None
-        dev = torch.device(self.device) if self.volume is not None else self.tsdf.device
+        dev = self.volume.device
         poses = packet["cam0_poses"].to(dev, torch.float32).contiguous()
         images = packet["cam0_images"]
         n, (H, W) = poses.shape[0], images.shape[-2:]
@@ -362,16 +410,8 @@ class TsdfFusion:
         with _lib.fixed_stream():
             for s in range(0, n, chunk):
                 m = min(chunk, n - s)
-                if self.volume is not None:
-                    depth[s:s + m], color[s:s + m] = self.volume.raycast(
-                        poses[s:s + m], H, W, intr, self.min_depth, self.max_depth, self.sdf_trunc, min_weight_for_render)[:2]
-                else:
-                    nz, ny, nx = self.tsdf.shape
-                    _lib.check(_lib.load().nslam_tsdf_raycast(
-                        _lib.ptr(self.tsdf), _lib.ptr(self.weight), _lib.ptr(self.color), nx, ny, nz, self.origin.ctypes.data,
-                        float(self.voxel_size), _lib.ptr(poses[s:s + m]), m, H, W, intr.ctypes.data, float(self.min_depth),
-                        float(self.max_depth), float(self.sdf_trunc), float(min_weight_for_render), _lib.ptr(depth[s:s + m]),
-                        _lib.ptr(color[s:s + m]), _lib.ptr(weight), None, _lib.stream_ptr()), "tsdf_raycast")
+                self.volume.raycast(poses[s:s + m], H, W, intr, self.min_depth, self.max_depth, self.sdf_trunc,
+                                    min_weight_for_render, depth=depth[s:s + m], color=color[s:s + m], weight=weight[:m])
                 if evaluate:
                     for i in range(s, s + m):
                         total_psnr += color_psnr(color[i], images[i])

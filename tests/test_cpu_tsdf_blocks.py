@@ -196,15 +196,16 @@ def test_growth_keeps_indices_and_order(monkeypatch):
     assert small.memory_bytes() > small.capacity * 80 * 1024
 
 
-def test_tsdf_fusion_dispatches_to_the_block_volume(monkeypatch):
+def test_tsdf_fusion_holds_one_volume_of_either_kind(monkeypatch):
     from nerf_slam_b200 import tsdf_blocks as tb
-    from nerf_slam_b200.tsdf_fusion import TsdfFusion
+    from nerf_slam_b200.tsdf_fusion import DenseVolume, TsdfFusion
     monkeypatch.setattr(tb.VoxelBlockVolume, "kernels", OracleKernels())
     with pytest.raises(ValueError):
         TsdfFusion("sigma", types.SimpleNamespace(tsdf_volume="hashed"), "cpu")
     args = types.SimpleNamespace(eval=False, tsdf_volume="blocks", tsdf_block_count=3)
     fus = TsdfFusion("sigma", args, "cpu")
-    assert fus.volume.capacity == 3 and not hasattr(fus, "tsdf")
+    assert isinstance(fus.volume, tb.VoxelBlockVolume) and fus.volume.capacity == 3
+    assert not any(hasattr(fus, a) for a in ("tsdf", "weight", "color", "origin"))
     fr = _frames(2)
     packet = {"cam0_poses": torch.stack([f[4] for f in fr]), "cam0_idepths_up": torch.stack([f[0] for f in fr]),
               "cam0_depths_cov_up": torch.stack([f[1] for f in fr]), "cam0_images": torch.stack([f[2] for f in fr])}
@@ -221,4 +222,29 @@ def test_tsdf_fusion_dispatches_to_the_block_volume(monkeypatch):
     assert fus.voxel_size == vs / 2 and fus.volume.voxel_size == float(np.float32(vs / 2))
     assert fus.volume.n_blocks == 0 and fus.volume.capacity == cap
     dense = TsdfFusion("sigma", types.SimpleNamespace(eval=False, tsdf_resolution=8), "cpu")
-    assert dense.volume is None and dense.tsdf.shape == (8, 8, 8)
+    assert isinstance(dense.volume, DenseVolume) and dense.volume.tsdf.shape == (8, 8, 8)
+    assert not any(hasattr(dense, a) for a in ("tsdf", "weight", "color", "origin"))
+
+
+def test_dense_volume_resets_in_place():
+    """reset_volume zeroes the dense grid's own tensors (no second grid) and moves the origin to the halved voxel"""
+    from nerf_slam_b200.tsdf_fusion import DenseVolume, TsdfFusion
+    centre = np.array([0.31, -0.52, 1.07], np.float32)
+    fus = TsdfFusion("sigma", types.SimpleNamespace(eval=False, tsdf_resolution=8, tsdf_center=tuple(centre)), "cpu")
+    vol = fus.volume
+    assert isinstance(vol, DenseVolume) and vol.device == "cpu" and vol.voxel_size == float(np.float32(6.0 / 512))
+    lattice = lambda vs: ((np.round(centre / np.float32(vs)) - 4) * np.float32(vs)).astype(np.float32)
+    assert vol.origin.dtype == np.float32 and np.array_equal(vol.origin, lattice(6.0 / 512))
+    assert vol.color.shape == (8, 8, 8, 3) and all(not t.any() for t in (vol.tsdf, vol.weight, vol.color))
+    assert vol.memory_bytes() == 8 ** 3 * 5 * 4
+    tensors = (vol.tsdf, vol.weight, vol.color)
+    ptrs = [t.data_ptr() for t in tensors]
+    for t in tensors:
+        t.fill_(1.5)
+    fus.reset_volume()
+    assert fus.volume is vol and fus.voxel_size == 3.0 / 512 and vol.voxel_size == float(np.float32(3.0 / 512))
+    assert all(a is b for a, b in zip((vol.tsdf, vol.weight, vol.color), tensors))
+    assert [t.data_ptr() for t in tensors] == ptrs and all(not t.any() for t in tensors)
+    assert np.array_equal(vol.origin, lattice(3.0 / 512)) and not np.array_equal(lattice(3.0 / 512), lattice(6.0 / 512))
+    t, w, c, org = vol.to_dense()
+    assert t is vol.tsdf and w is vol.weight and c is vol.color and org is vol.origin

@@ -25,7 +25,7 @@ def _args(dataset_dir, fusion, buffer=24):
 
 
 @pytest.mark.parametrize("fusion", ["nerf", "sigma"])
-def test_reference_pipeline_wiring_on_hardware(tmp_path, monkeypatch, fusion):
+def test_reference_pipeline_wiring_and_fusion_volume_on_hardware(tmp_path, monkeypatch, fusion):
     from nerf_slam_b200 import datasets, synthetic
     room = synthetic.SyntheticRoom(320, 240, 56, seed=0, step=0.03)
     datasets.write_transforms_dataset(room, str(tmp_path))
@@ -58,4 +58,4 @@ def test_reference_pipeline_wiring_on_hardware(tmp_path, monkeypatch, fusion):
     else:
         vol = fus.fusion
         assert vol.integrated_frames >= 9 and len(vol.history) >= 9
-        assert float((vol.weight > 0).float().mean()) > 0.01 and torch.isfinite(vol.tsdf).all()
+        assert float((vol.volume.weight > 0).float().mean()) > 0.01 and torch.isfinite(vol.volume.tsdf).all()

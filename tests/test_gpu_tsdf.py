@@ -95,7 +95,7 @@ def test_tsdf_kernel_matches_the_reference_methods_executed_verbatim(tag, mw):
             assert np.allclose(gw, rw, rtol=3e-7, atol=0) and np.allclose(gt, rt, rtol=0, atol=3e-7) and np.allclose(gc, rc, rtol=0, atol=1e-4), k
 
 
-def test_tsdf_fusion_of_ground_truth_packets_recovers_the_room():
+def test_tsdf_fusion_volume_of_ground_truth_packets_recovers_the_room():
     """TsdfFusion('sigma') fed SLAM-shaped packets built from the synthetic room's ground-truth poses and depths: the
     zero crossings of the fused TSDF lie on the room's walls (within two voxels), history / rebuild work"""
     from nerf_slam_b200.synthetic import SyntheticRoom
@@ -126,7 +126,7 @@ def test_tsdf_fusion_of_ground_truth_packets_recovers_the_room():
     dist_to_wall = (he - pts.abs()).abs().min(dim=1).values
     assert float((dist_to_wall < 2.5 * fus.voxel_size).float().mean()) > 0.97
     assert float(cols.mean()) > 5.0                                                # colours were fused (u8 scale)
-    w0 = float(fus.weight.sum())
+    w0 = float(fus.volume.weight.sum())
     fus.rebuild_volume()                                                           # history -> fresh volume at half the voxel size (:304-316)
     torch.cuda.synchronize()
-    assert fus.voxel_size == pytest.approx(8.0 / 512) and float(fus.weight.sum()) > 0 and w0 > 0
+    assert fus.voxel_size == pytest.approx(8.0 / 512) and float(fus.volume.weight.sum()) > 0 and w0 > 0

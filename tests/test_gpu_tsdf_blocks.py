@@ -184,14 +184,12 @@ def _canonical_triangles(v, tri):
     return out
 
 
-def test_mesh_equals_the_dense_mesh_of_the_embedding():
-    from nerf_slam_b200.tsdf_fusion import TsdfFusion
+def test_block_mesh_equals_the_dense_volume_mesh_of_the_embedding():
+    from nerf_slam_b200.tsdf_fusion import DenseVolume
     vol = _fused()
     mesh = vol.build_mesh(0.5)
     t, w, c = _embed0(vol)
-    fus = TsdfFusion("tsdf", types.SimpleNamespace(eval=False, tsdf_resolution=2), DEV)
-    fus.tsdf, fus.weight, fus.color, fus.origin, fus.voxel_size = t, w, c, np.zeros(3, F32), vol.voxel_size
-    dense = fus.build_mesh(0.5)
+    dense = DenseVolume.from_tensors(t, w, c, np.zeros(3, F32), vol.voxel_size).build_mesh(0.5)
     torch.cuda.synchronize()
     v, dv = mesh.vertices.cpu().numpy(), dense.vertices.cpu().numpy()
     assert v.shape == dv.shape and mesh.triangles.shape == dense.triangles.shape and len(v) > 1000

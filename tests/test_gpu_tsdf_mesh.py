@@ -18,11 +18,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 def _fusion(t, w, c, origin, vs):
-    from nerf_slam_b200.tsdf_fusion import TsdfFusion
+    from nerf_slam_b200.tsdf_fusion import DenseVolume, TsdfFusion
     fus = TsdfFusion("tsdf", types.SimpleNamespace(eval=False, tsdf_resolution=2), DEV)
     T = lambda a: torch.from_numpy(np.ascontiguousarray(a, F32)).to(DEV)
-    fus.tsdf, fus.weight, fus.color = T(t), T(w), T(c)
-    fus.origin, fus.voxel_size = np.asarray(origin, F32), float(vs)
+    fus.volume, fus.voxel_size = DenseVolume.from_tensors(T(t), T(w), T(c), origin, vs), float(vs)
     return fus
 
 
@@ -61,7 +60,7 @@ MIN_W = 0.5
 
 
 @pytest.mark.parametrize("name", sorted(VOLUMES))
-def test_mesh_matches_oracle(name):
+def test_dense_volume_mesh_matches_oracle(name):
     t, w, c, origin, vs = VOLUMES[name]()
     V, T, C, N = orc.marching_cubes(t, w, c, origin, vs, MIN_W)
     assert len(T) > 50
@@ -106,7 +105,7 @@ def _poses(origin, vs, shape, rng, n):
 def test_raycast_matches_oracle(name):
     from nerf_slam_b200 import _lib
     t, w, c, origin, vs = VOLUMES[name]()
-    fus = _fusion(t, w, c, origin, vs)
+    vol = _fusion(t, w, c, origin, vs).volume
     lib = _lib.load()
     if name.startswith("golden"):
         # the golden volume is observed only from its own three keyframes (30 x 40, fx = 22): view it from those
@@ -123,8 +122,8 @@ def test_raycast_matches_oracle(name):
         d_tq = torch.from_numpy(np.stack(tqs)).to(DEV)
         out = [torch.empty(n, H, W, device=DEV), torch.empty(n, H, W, 3, device=DEV), torch.empty(n, H, W, device=DEV),
                torch.empty(n, H, W, 3, device=DEV)]
-        _lib.check(lib.nslam_tsdf_raycast(_lib.ptr(fus.tsdf), _lib.ptr(fus.weight), _lib.ptr(fus.color), t.shape[2], t.shape[1],
-                                          t.shape[0], fus.origin.ctypes.data, vs, _lib.ptr(d_tq), n, H, W, intr.ctypes.data,
+        _lib.check(lib.nslam_tsdf_raycast(_lib.ptr(vol.tsdf), _lib.ptr(vol.weight), _lib.ptr(vol.color), t.shape[2], t.shape[1],
+                                          t.shape[0], vol.origin.ctypes.data, vs, _lib.ptr(d_tq), n, H, W, intr.ctypes.data,
                                           0.01, 6.0, 0.10, 0.01, *[_lib.ptr(o) for o in out], _lib.stream_ptr()), "raycast")
         torch.cuda.synchronize()
         gd, gc, gw, gn = [o.cpu().numpy() for o in out]
@@ -223,7 +222,7 @@ def test_gui_packet_builds_a_mesh_and_writes_results_csv(room_fusion, tmp_path, 
     assert np.isfinite(psnr) and np.isfinite(l1) and psnr > PSNR_MIN and l1 < 10.0
 
 
-def test_mesh_scratch_grows_with_the_surface_not_the_grid():
+def test_dense_volume_mesh_scratch_grows_with_the_surface_not_the_grid():
     from nerf_slam_b200.synthetic import SyntheticRoom
     from nerf_slam_b200.tsdf_fusion import TsdfFusion
     room = SyntheticRoom(W, H, 40, seed=0)
@@ -232,7 +231,7 @@ def test_mesh_scratch_grows_with_the_surface_not_the_grid():
     for _, pkt in _room_packets(room, range(0, 40, 8)):
         fus.fuse({"slam": [None, pkt]})
     torch.cuda.synchronize()
-    volume_bytes = sum(x.numel() * x.element_size() for x in (fus.tsdf, fus.weight, fus.color))
+    volume_bytes = fus.volume.memory_bytes()
     base = torch.cuda.memory_allocated()
     torch.cuda.reset_peak_memory_stats()
     mesh = fus.build_mesh(0.5)
