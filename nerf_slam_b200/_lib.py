@@ -105,6 +105,17 @@ _SIGNATURES = {
     "nslam_point_cloud_voxel_scratch": [c_int, _P],
     "nslam_point_cloud_voxel_sort": [_P, c_int, c_float, _P, ctypes.c_longlong, _P, _P],
     "nslam_point_cloud_voxel_reduce": [_P, _P, c_int, _P, ctypes.c_longlong, c_int, _P, _P, _P, _P],
+    # reconstruction evaluation (include/nslam_eval.h)
+    "nslam_eval_surface_scratch": [c_int, _P],
+    "nslam_eval_surface_area": [_P, c_int, _P, c_int, _P, ctypes.c_longlong, _P, _P],
+    "nslam_eval_sample_surface": [_P, _P, c_int, c_int, ctypes.c_ulonglong, _P, ctypes.c_longlong, _P, _P, _P],
+    "nslam_eval_bvh_scratch": [c_int, c_int, _P],
+    "nslam_eval_bvh_build": [_P, c_int, c_int, _P, ctypes.c_longlong, _P],
+    "nslam_eval_nearest_scratch": [c_int, _P],
+    "nslam_eval_nearest": [_P, ctypes.c_longlong, c_int, c_int, _P, c_int, c_float, c_int, _P, ctypes.c_longlong, _P, _P,
+                           _P],
+    "nslam_eval_visible": [_P, c_int, _P, c_int, _P, c_int, c_int, _P, c_float, c_float, c_float, _P, _P],
+    "nslam_eval_reduce": [_P, c_int, c_float, c_float, _P, _P],
     "nslam_ba_reduced_camera_matrix": [ctypes.POINTER(BAGraph), ctypes.POINTER(BABuffers), _P],
     "nslam_ba_tile_pixels": [],
     "nslam_ba_solve": [_P, _P, c_int, c_int, _P, c_float, c_float, c_float, _P, _P, _P, _P, _P],

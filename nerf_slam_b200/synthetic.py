@@ -130,6 +130,24 @@ class SyntheticRoom:
         d16 = np.clip(depth / self.calib.depth_scale, 0, 65535).astype(np.uint16).astype(np.int32)[..., None]
         return rgba, d16, np.linalg.inv(T)
 
+    def surface_mesh(self):
+        """the exact surface `render` ray-casts: the room's six faces at +-half_extent as 12 triangles -> vertices [8,3]
+        float32 (corner k at -ext / +ext per axis by bits 0, 1, 2 of k), triangles [12,3] int32 wound so that
+        (b - a) x (c - a) points into the room, i.e. into free space (the convention of TsdfMesh)"""
+        ext = self.ext.astype(np.float32)
+        k = np.arange(8)
+        vertices = np.stack([np.where((k >> a) & 1, ext[a], -ext[a]) for a in range(3)], 1).astype(np.float32)
+        tris = []
+        for a in range(3):
+            b, c = (a + 1) % 3, (a + 2) % 3
+            for side in (0, 1):
+                # corners (b, c) = (0,0), (1,0), (1,1), (0,1) of the face: counter-clockwise about +e_a
+                q = [side << a | i << b | j << c for i, j in ((0, 0), (1, 0), (1, 1), (0, 1))]
+                if side:                                   # the +ext face looks toward -e_a
+                    q = q[::-1]
+                tris += [(q[0], q[1], q[2]), (q[0], q[2], q[3])]
+        return vertices, np.asarray(tris, np.int32)
+
     def packet(self, k):
         rgba, d16, w2c = self.render(k)
         return {"k": np.arange(k, k + 1), "t_cams": np.array([k]), "poses": np.array([w2c]),
