@@ -30,6 +30,9 @@ typedef struct nslam_ngp_model {
   float aabb_scale; int cascades; float cone; float near_distance;
   float scale[16]; int res[16]; unsigned size[16]; unsigned offset[16]; int dense[16];
   unsigned n_grid;
+  long long* grid_grad_fx;  /* [n_grid*2]         fixed-point hash-grid gradient accumulator: zero on entry, zero on return */
+  float* mlp_grad_part;     /* [part_rows,10240]  per-CTA weight-gradient partials of the tensor-core backward       */
+  int part_rows;            /* rows of mlp_grad_part: nslam_ngp_backward_tc needs num_sms <= part_rows             */
 } nslam_ngp_model;
 
 typedef struct nslam_ngp_images {
@@ -52,6 +55,7 @@ typedef struct nslam_ngp_batch {
   int max_rays, max_samples;
   void* enc;         /* __half [max_samples,32]  hash encodings kept by the tensor-core forward (or NULL) */
   void* denc;        /* __half [max_samples,32]  loss-scaled encoding gradients for the scatter kernel (or NULL) */
+  long long* loss_fx; /* [1] fixed-point loss accumulator: zero on entry, zero on return */
 } nslam_ngp_batch;
 
 int nslam_ngp_train_step(const nslam_ngp_model* m, const nslam_ngp_images* im, const nslam_ngp_batch* b,
@@ -86,11 +90,12 @@ int nslam_ngp_ingest_batch(const unsigned char* rgb_chw, const float* idepth_up,
 
 /* Camera-pose refinement (`nerf.training.optimize_extrinsics`, fusion/nerf_fusion.py:99; csrc/ngp_extrinsics.cu):
  * gradient of the batch just back-propagated w.r.t. each camera's translation and rotation vector, accumulated into
- * cam_grad [n_images,6]; then Adam on the offsets [n_images,6] and the effective cameras the sampler reads. */
+ * cam_grad [n_images,6] through the fixed-point cam_grad_fx [n_images,6] (zero on entry, zero on return); then Adam on
+ * the offsets [n_images,6] and the effective cameras the sampler reads. */
 int nslam_ngp_cam_grad(const void* grid_half, const float* scale16, const int* res16, const unsigned* size16,
                        const unsigned* offset16, const int* dense16, float aabb_scale, const float* rays, int max_rays,
                        const float* coords, const float* tdist, const void* denc, float loss_scale, float* cam_grad,
-                       int n_images, void* stream);
+                       long long* cam_grad_fx, int n_images, void* stream);
 int nslam_ngp_cam_adam_apply(const void* base_cams, void* eff_cams, float* offsets, float* cam_grad, float* m, float* v,
                              int* steps, int n, float lr, float beta1, float beta2, float eps, float l2, void* stream);
 
@@ -105,7 +110,7 @@ int nslam_ngp_forward_tc(const nslam_ngp_model* m, const void* packed, const flo
                          int n, int max_samples, float* rgbsigma, void* enc_out, int num_sms, void* stream);
 /* enc_in (from forward_tc's enc_out) or NULL = re-gather; denc_scratch or NULL = scatter inside the kernel.
  * With denc_scratch the hash-grid scatter runs as its own full-occupancy kernel (one thread per
- * sample x level) after the MLP backward. */
+ * sample x level) after the MLP backward.  cudaErrorInvalidValue when num_sms > m->part_rows. */
 int nslam_ngp_backward_tc(const nslam_ngp_model* m, const void* packed, const float* coords, const int* counters,
                           const float* dout, float loss_scale, const void* enc_in, void* denc_scratch,
                           int max_samples, int num_sms, void* stream);
@@ -120,12 +125,13 @@ int nslam_ngp_loss_backward_tc(const nslam_ngp_model* m, const nslam_ngp_batch* 
  * tensor-core density head (encode -> layers 1-2) -> field = thresh - sigma (negative inside), weight = 1 where the
  * point's occupancy cell (cascade of the finest box holding it) was seen by a training camera, else 0 [nz,ny,nx] fp32
  * (DEVICE); marching cubes of nslam_tsdf_mesh_* with min_weight 0 and color NULL follow.  _colors: colors [n,3] = network
- * radiance at the vertices [n,3] seen along -normals [n,3] (+z where the normal is 0), through the tensor-core forward;
- * srgb != 0: encoded with the inverse of the ingest's sRGB -> linear curve.  `packed` as for forward_tc. */
+ * radiance at the vertices [n,3] seen along -normals [n,3] (+z where the normal is 0), through the tensor-core forward in
+ * chunks of 2^18 vertices; srgb != 0: encoded with the inverse of the ingest's sRGB -> linear curve.  scratch: DEVICE,
+ * scratch_bytes >= 44 * min(n, 2^18).  `packed` as for forward_tc. */
 int nslam_ngp_mesh_lattice(const nslam_ngp_model* m, const void* packed, const float* lo3_host, float h, int nx, int ny,
                            int nz, float thresh, float* field, float* weight, int num_sms, void* stream);
 int nslam_ngp_mesh_colors(const nslam_ngp_model* m, const void* packed, const float* vertices, const float* normals, int n,
-                          int srgb, float* colors, int num_sms, void* stream);
+                          int srgb, float* colors, void* scratch, long long scratch_bytes, int num_sms, void* stream);
 /* the non-network phases of a step (shared by both variants) */
 int nslam_ngp_sample_phase(const nslam_ngp_model* m, const nslam_ngp_images* im, const nslam_ngp_batch* b,
                            int n_rays, unsigned seed, void* stream);

@@ -144,7 +144,7 @@ _SIGNATURES = {
     "nslam_ngp_ingest_image": [_P, _P, _P, c_int, c_int, _P, _P, _P, _P],
     "nslam_ngp_ingest_batch": [_P, _P, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P, c_float, c_float, c_float, c_float, _P, _P,
                                _P, _P, c_int, _P],
-    "nslam_ngp_cam_grad": [_P, _P, _P, _P, _P, _P, c_float, _P, c_int, _P, _P, _P, c_float, _P, c_int, _P],
+    "nslam_ngp_cam_grad": [_P, _P, _P, _P, _P, _P, c_float, _P, c_int, _P, _P, _P, c_float, _P, _P, c_int, _P],
     "nslam_ngp_cam_adam_apply": [_P, _P, _P, _P, _P, _P, _P, c_int, c_float, c_float, c_float, c_float, c_float, _P],
     "nslam_ngp_pack_mlp": [_P, _P, _P],
     "nslam_ngp_forward_tc": [_P, _P, _P, _P, c_int, c_int, _P, _P, c_int, _P],
@@ -154,7 +154,7 @@ _SIGNATURES = {
     "nslam_ngp_sample_phase": [_P, _P, _P, c_int, ctypes.c_uint, _P],
     "nslam_ngp_loss_phase": [_P, c_int, c_float, c_float, c_float, c_float, _P],
     "nslam_ngp_mesh_lattice": [_P, _P, _P, c_float, c_int, c_int, c_int, c_float, _P, _P, c_int, _P],
-    "nslam_ngp_mesh_colors": [_P, _P, _P, _P, c_int, c_int, _P, c_int, _P],
+    "nslam_ngp_mesh_colors": [_P, _P, _P, _P, c_int, c_int, _P, _P, ctypes.c_longlong, c_int, _P],
     # tensor-core convolution (include/nslam_nn.h)
     "nslam_conv_igemm": [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int,
                          _P, _P, _P, _P, _P, c_int, _P, _P, c_int, _P],
@@ -189,6 +189,13 @@ def load(require_cuda=True):
                                    "there is no CPU fallback")
         _cuda_ok = True          # checked once: the query costs ~4 us and every operator comes through here
     return _lib
+
+
+def query_size(name, *args):
+    """the size (bytes or an element count) that the C query `name(*args, long long* out)` writes; raises on an error"""
+    out = ctypes.c_longlong(0)
+    check(getattr(load(), name)(*args, ctypes.byref(out)), name)
+    return out.value
 
 
 def check(err, what):

@@ -19,7 +19,6 @@
 //    (deterministic order, fp64 accumulation like the reference's Eigen path), factorised by a
 //    single-CTA fp64 Cholesky (n <= 168 in shared memory) and the SE3/inverse-depth updates
 //    follow on the same stream.
-#include <atomic>
 #include "common.cuh"
 #include "../../include/nslam_ba.h"
 
@@ -758,23 +757,6 @@ __global__ void ba_pose_cov_kernel(const float* __restrict__ Linv, int P, float*
 
 }  // namespace nslam
 
-namespace nslam {
-// cudaFuncAttributeMaxDynamicSharedMemorySize is a PER-DEVICE attribute: remember what was configured per device
-// (a process may drive several GPUs, or reset one) instead of once per process
-template <typename K>
-static cudaError_t ensure_dyn_smem(K kernel, size_t smem, std::atomic<size_t>* cache /* [NSLAM_MAX_DEVICES] */) {
-  if (smem <= 48 * 1024) return cudaSuccess;
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  if (dev < 0 || dev >= NSLAM_MAX_DEVICES) dev = NSLAM_MAX_DEVICES - 1, cache[dev] = 0;   // overflow slot: always set
-  if (smem <= cache[dev].load(std::memory_order_acquire)) return cudaSuccess;
-  e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e == cudaSuccess) cache[dev].store(smem, std::memory_order_release);
-  return e;
-}
-}  // namespace nslam
-
 extern "C" {
 
 int nslam_ba_reduced_camera_matrix(const nslam_ba_graph* g, const nslam_ba_buffers* b,
@@ -795,11 +777,7 @@ int nslam_ba_reduced_camera_matrix(const nslam_ba_graph* g, const nslam_ba_buffe
   }
   const size_t smem = ((size_t)6 * g->RMAX * (TILE + 1) + 2 * TILE) * sizeof(float);
   if (smem > 227 * 1024) return (int)cudaErrorInvalidValue;
-  static std::atomic<size_t> configured[NSLAM_MAX_DEVICES];
-  {
-    cudaError_t e = ensure_dyn_smem(ba_schur_kernel, smem, configured);
-    if (e != cudaSuccess) return (int)e;
-  }
+  if (cudaError_t e = ensure_dyn_smem<ba_schur_kernel>(smem)) return (int)e;
   ba_schur_kernel<<<grid, TILE, smem, st>>>(*g, *b);
   NSLAM_CHECK_LAUNCH();
   const int nvals = g->NPAIR * 36 + g->NR * 6;
@@ -819,9 +797,7 @@ static int launch_solve(const float* Hin, const float* vin, int P, int prior_pos
   const int n = 6 * P;
   const size_t smem = (size_t)n * n * sizeof(double);
   if (smem <= 200 * 1024) {
-    static std::atomic<size_t> configured[NSLAM_MAX_DEVICES];
-    cudaError_t e = ensure_dyn_smem(ba_solve_kernel<true>, smem > 48 * 1024 ? (size_t)200 * 1024 : smem, configured);
-    if (e != cudaSuccess) return (int)e;
+    if (cudaError_t e = ensure_dyn_smem<ba_solve_kernel<true>>(smem > 48 * 1024 ? (size_t)200 * 1024 : smem)) return (int)e;
     ba_solve_kernel<true><<<1, 256, smem, st>>>(Hin, vin, n, prior_pose_idx, prior_err, prior_info,
                                                 lm, ep, work, dx, Linv, status, fail_count);
   } else {
@@ -881,11 +857,7 @@ int nslam_ba_cov(const nslam_ba_graph* g, const nslam_ba_buffers* b, const float
   NSLAM_CHECK_LAUNCH();
   const size_t smem = (size_t)g->RMAX * g->RMAX * 36 * sizeof(float);
   if (smem > 227 * 1024) return (int)cudaErrorInvalidValue;
-  static std::atomic<size_t> configured[NSLAM_MAX_DEVICES];
-  {
-    cudaError_t e = ensure_dyn_smem(ba_cov_kernel, smem, configured);
-    if (e != cudaSuccess) return (int)e;
-  }
+  if (cudaError_t e = ensure_dyn_smem<ba_cov_kernel>(smem)) return (int)e;
   dim3 grid(b->T, g->K);
   ba_cov_kernel<<<grid, TILE, smem, st>>>(*g, *b, Mscratch, z_cov, depth_cov);
   NSLAM_CHECK_LAUNCH();

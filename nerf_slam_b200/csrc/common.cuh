@@ -8,6 +8,7 @@
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
 #include <stdint.h>
+#include <atomic>
 
 #define NSLAM_MIN_DEPTH 0.25f   // src/droid_kernels.cu:26
 #define NSLAM_MAX_DEVICES 64    // per-device caches of kernel attributes (last slot = overflow: always re-set)
@@ -19,6 +20,37 @@
   } while (0)
 
 namespace nslam {
+
+// Lets `Kernel` launch with `smem` bytes of dynamic shared memory.  cudaFuncAttributeMaxDynamicSharedMemorySize is a
+// PER-DEVICE attribute, so what was configured is remembered per device (a process may drive several GPUs, or reset
+// one) instead of once per process; each instantiation owns its cache.
+template <auto Kernel>
+inline cudaError_t ensure_dyn_smem(size_t smem) {
+  static std::atomic<size_t> cache[NSLAM_MAX_DEVICES];
+  if (smem <= 48 * 1024) return cudaSuccess;
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev < 0 || dev >= NSLAM_MAX_DEVICES) dev = NSLAM_MAX_DEVICES - 1, cache[dev] = 0;   // overflow slot: always set
+  if (smem <= cache[dev].load(std::memory_order_acquire)) return cudaSuccess;
+  e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e == cudaSuccess) cache[dev].store(smem, std::memory_order_release);
+  return e;
+}
+
+// Lays out caller-owned scratch: take(bytes) hands out consecutive regions, each starting 256-byte aligned.  With a
+// null base only the total `off` is computed (the size query) and every pointer is null.
+struct ScratchCarver {
+  char* base;
+  size_t off = 0;
+  explicit ScratchCarver(void* b) : base((char*)b) {}
+  template <typename T = void>
+  T* take(size_t bytes) {
+    T* p = base ? (T*)(base + off) : nullptr;
+    off += (bytes + 255) & ~(size_t)255;
+    return p;
+  }
+};
 
 struct Intr { float fx, fy, cx, cy; };
 

@@ -1,7 +1,6 @@
 // Shared pieces of the implicit-GEMM convolution kernel (conv_igemm.cu): launch parameters, shared-memory plan,
 // epilogue math.
 #pragma once
-#include <atomic>
 #include "common.cuh"
 #include "tc.cuh"
 

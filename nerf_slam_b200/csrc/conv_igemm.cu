@@ -373,12 +373,7 @@ conv_partials_reduce_kernel(const float* __restrict__ partials, float* __restric
 template <int N, int MODE, bool HALO>
 static int launch_conv_mh(const ConvMaps& maps, const ConvParams& p, int num_sms, cudaStream_t st) {
   const int smem = CgSmem<N, HALO>::TOTAL + 1024;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(conv_igemm_kernel<N, MODE, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return (int)e;
-    configured = true;
-  }
+  if (cudaError_t e = ensure_dyn_smem<conv_igemm_kernel<N, MODE, HALO>>(smem)) return (int)e;
   const int ntiles = p.B * p.tiles_h * p.tiles_w;
   const int grid = ntiles < num_sms ? ntiles : num_sms;
   conv_igemm_kernel<N, MODE, HALO><<<grid, CG_THREADS, smem, st>>>(maps, p);

@@ -373,13 +373,7 @@ int nslam_corr_volume_build(const void* fmaps, int NF, int H, int W, int C, cons
   }
   p.tma_l0 = use_tma[0]; p.tma_l1 = use_tma[1];
   const int smem = CvSmem::TOTAL + 1024;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t er = cudaFuncSetAttribute(corr_volume_tc_kernel,
-                                          cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (er != cudaSuccess) return (int)er;
-    configured = true;
-  }
+  if (cudaError_t e = ensure_dyn_smem<corr_volume_tc_kernel>(smem)) return (int)e;
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);

@@ -280,12 +280,7 @@ static int launch_rows(const void* fmaps, int NF, int H, const int* ii, const in
   p.split = (p.RP + p.rp_chunk - 1) / p.rp_chunk;
   p.nwork = E * p.MT * p.split;
   const int smem = SM::TOTAL + 1024;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t er = cudaFuncSetAttribute(corr_volume_rows_kernel<W2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (er != cudaSuccess) return (int)er;
-    configured = true;
-  }
+  if (cudaError_t e = ensure_dyn_smem<corr_volume_rows_kernel<W2>>(smem)) return (int)e;
   const int grid = p.nwork < sms ? p.nwork : sms;
   corr_volume_rows_kernel<W2><<<grid, CR_THREADS, smem, st>>>(tmA, tmB, tmO0, tmO1, p);
   NSLAM_CHECK_LAUNCH();

@@ -6,6 +6,8 @@
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
 #include <stdint.h>
+#include "common.cuh"
+#include "../../include/nslam_ngp.h"
 
 namespace ngp {
 
@@ -37,6 +39,15 @@ struct LevelInfo {
   uint32_t offset[N_LEVELS];  // entry offset of level
   int dense[N_LEVELS];        // res^3 <= size
 };
+
+static inline LevelInfo level_info(const nslam_ngp_model* m) {
+  LevelInfo lv;
+  for (int l = 0; l < N_LEVELS; l++) {
+    lv.scale[l] = m->scale[l]; lv.res[l] = m->res[l]; lv.size[l] = m->size[l];
+    lv.offset[l] = m->offset[l]; lv.dense[l] = m->dense[l];
+  }
+  return lv;
+}
 
 struct Camera {      // per training image
   float c2w[12];     // 3x4 row-major
@@ -185,22 +196,3 @@ static __global__ void fx_flush_kernel(long long* __restrict__ acc, float* __res
   }
 }
 }  // namespace ngp
-
-// library-owned device scratch, one buffer per (device, slot), grown on demand and zero-filled when (re)allocated
-inline void* ngp_scratch(int slot, size_t bytes) {
-  static void* ptr[64][5] = {};
-  static size_t cap[64][5] = {};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64 || slot < 0 || slot >= 5) return nullptr;
-  if (cap[dev][slot] < bytes) {
-    if (ptr[dev][slot]) cudaFree(ptr[dev][slot]);
-    ptr[dev][slot] = nullptr; cap[dev][slot] = 0;
-    if (cudaMalloc(&ptr[dev][slot], bytes) != cudaSuccess) { ptr[dev][slot] = nullptr; return nullptr; }
-    cudaMemset(ptr[dev][slot], 0, bytes);
-    cap[dev][slot] = bytes;
-  }
-  return ptr[dev][slot];
-}
-enum { NGP_SCRATCH_GRID = 0, NGP_SCRATCH_DW = 1, NGP_SCRATCH_CAM = 2, NGP_SCRATCH_LOSS = 3, NGP_SCRATCH_MESH = 4 };
-

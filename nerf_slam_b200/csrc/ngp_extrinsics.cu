@@ -15,12 +15,6 @@
 // One WARP per ray (lanes = samples), table gathers from the L2-resident fp16 grid, one atomic per ray and component.
 #include "ngp_common.cuh"
 
-#define NGX_CHECK_LAUNCH()                           \
-  do {                                               \
-    cudaError_t e__ = cudaGetLastError();            \
-    if (e__ != cudaSuccess) return (int)e__;         \
-  } while (0)
-
 namespace ngp {
 
 struct ExtrLevels {
@@ -152,27 +146,26 @@ __global__ void cam_adam_apply_kernel(const Camera* __restrict__ base, Camera* _
 extern "C" {
 
 /* dL/d(camera) of the batch just back-propagated (rays / coords / tdist / denc of nslam_ngp_batch after
- * nslam_ngp_train_step_tc) accumulated into cam_grad [n_images,6] = (d translation, d rotation vector).
+ * nslam_ngp_train_step_tc) accumulated into cam_grad [n_images,6] = (d translation, d rotation vector) through the
+ * fixed-point accumulator cam_grad_fx [n_images,6] (zero on entry, zero on return).
  * grid_half / level tables as in nslam_ngp_model; loss_scale = the scale the backward applied to denc. */
 int nslam_ngp_cam_grad(const void* grid_half, const float* scale16, const int* res16, const unsigned* size16,
                        const unsigned* offset16, const int* dense16, float aabb_scale, const float* rays, int max_rays,
                        const float* coords, const float* tdist, const void* denc, float loss_scale, float* cam_grad,
-                       int n_images, void* stream) {
+                       long long* cam_grad_fx, int n_images, void* stream) {
   using namespace ngp;
   ExtrLevels lv;
   for (int l = 0; l < N_LEVELS; l++) {
     lv.scale[l] = scale16[l]; lv.res[l] = res16[l]; lv.size[l] = size16[l]; lv.offset[l] = offset16[l]; lv.dense[l] = dense16[l];
   }
   if (max_rays <= 0 || n_images <= 0) return 0;
-  long long* acc = (long long*)ngp_scratch(NGP_SCRATCH_CAM, (size_t)n_images * 6 * sizeof(long long));
-  if (!acc) return (int)cudaErrorMemoryAllocation;
   const int threads = 256, warps_per_block = threads / 32;
   cam_grad_kernel<<<(max_rays + warps_per_block - 1) / warps_per_block, threads, 0, (cudaStream_t)stream>>>(
       rays, max_rays, coords, tdist, (const __half*)denc, (const __half2*)grid_half, lv, 1.f / aabb_scale, 1.f / loss_scale,
-      acc);
-  NGX_CHECK_LAUNCH();
-  fx_flush_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(acc, cam_grad, (size_t)n_images * 6, 1.f / CAM_FX);
-  NGX_CHECK_LAUNCH();
+      cam_grad_fx);
+  NSLAM_CHECK_LAUNCH();
+  fx_flush_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(cam_grad_fx, cam_grad, (size_t)n_images * 6, 1.f / CAM_FX);
+  NSLAM_CHECK_LAUNCH();
   return 0;
 }
 
@@ -183,7 +176,7 @@ int nslam_ngp_cam_adam_apply(const void* base_cams, void* eff_cams, float* offse
   if (n <= 0) return 0;
   ngp::cam_adam_apply_kernel<<<(n + 63) / 64, 64, 0, (cudaStream_t)stream>>>(
       (const ngp::Camera*)base_cams, (ngp::Camera*)eff_cams, offsets, cam_grad, m, v, steps, n, lr, beta1, beta2, eps, l2);
-  NGX_CHECK_LAUNCH();
+  NSLAM_CHECK_LAUNCH();
   return 0;
 }
 

@@ -808,33 +808,25 @@ int nslam_ngp_pack_mlp(const float* mlp, void* packed, void* stream) {
   ngp::pack_mlp_kernel<<<(total + 255) / 256, 256, 0, (cudaStream_t)stream>>>(mlp, (unsigned char*)packed);
   const int totalb = (64 + 64 + 32 + 64 + 32) * 64;
   ngp::pack_mlp_bwd_kernel<<<(totalb + 255) / 256, 256, 0, (cudaStream_t)stream>>>(mlp, (unsigned char*)packed + ngp::PW_TOTAL);
-  return (int)cudaGetLastError();
+  NSLAM_CHECK_LAUNCH();
+  return 0;
 }
 
 /* tensor-core variant of nslam_ngp_forward: coords [n,7] (n < 0: read counters[0]) -> rgbsigma [n,4] */
 int nslam_ngp_forward_tc(const nslam_ngp_model* m, const void* packed, const float* coords, const int* counters,
                          int n, int max_samples, float* rgbsigma, void* enc_out, int num_sms, void* stream) {
   using namespace ngp;
-  LevelInfo lv;
-  for (int l = 0; l < N_LEVELS; l++) {
-    lv.scale[l] = m->scale[l]; lv.res[l] = m->res[l]; lv.size[l] = m->size[l];
-    lv.offset[l] = m->offset[l]; lv.dense[l] = m->dense[l];
-  }
   const int smem = FwdSmem::TOTAL + 1024;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(forward_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return (int)e;
-    configured = true;
-  }
+  if (cudaError_t e = nslam::ensure_dyn_smem<forward_tc_kernel>(smem)) return (int)e;
   const int cap = n >= 0 ? n : max_samples;
   if (cap == 0) return 0;
   int grid = (cap + 127) / 128;
   if (grid > 4 * num_sms) grid = 4 * num_sms;
-  forward_tc_kernel<<<grid, 128, smem, (cudaStream_t)stream>>>(coords, counters, n, (const __half2*)m->grid_half, lv,
-                                                              (const unsigned char*)packed, rgbsigma, (__half*)enc_out);
-  cudaError_t e = cudaGetLastError();
-  return (int)e;
+  forward_tc_kernel<<<grid, 128, smem, (cudaStream_t)stream>>>(coords, counters, n, (const __half2*)m->grid_half,
+                                                              level_info(m), (const unsigned char*)packed, rgbsigma,
+                                                              (__half*)enc_out);
+  NSLAM_CHECK_LAUNCH();
+  return 0;
 }
 
 /* tensor-core backward: recompute + all gradients; reads the sample count from counters[0].
@@ -843,44 +835,30 @@ int nslam_ngp_backward_tc(const nslam_ngp_model* m, const void* packed,
                           const float* coords, const int* counters, const float* dout, float loss_scale,
                           const void* enc_in, void* denc_scratch, int max_samples, int num_sms, void* stream) {
   using namespace ngp;
-  LevelInfo lv;
-  for (int l = 0; l < N_LEVELS; l++) {
-    lv.scale[l] = m->scale[l]; lv.res[l] = m->res[l]; lv.size[l] = m->size[l];
-    lv.offset[l] = m->offset[l]; lv.dense[l] = m->dense[l];
-  }
+  if (num_sms > m->part_rows) return (int)cudaErrorInvalidValue;
   const int smem = BwdSmem::TOTAL + 1024;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(backward_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return (int)e;
-    configured = true;
-  }
+  if (cudaError_t e = nslam::ensure_dyn_smem<backward_tc_kernel>(smem)) return (int)e;
+  const LevelInfo lv = level_info(m);
   cudaStream_t st = (cudaStream_t)stream;
-  float* dw_part = (float*)ngp_scratch(NGP_SCRATCH_DW, (size_t)num_sms * W_TOTAL * sizeof(float));
-  if (!dw_part) return (int)cudaErrorMemoryAllocation;
   backward_tc_kernel<<<num_sms, 128, smem, st>>>(coords, counters, (const __half2*)m->grid_half, lv,
                                                  (const unsigned char*)packed, (const unsigned char*)packed + PW_TOTAL,
-                                                 dout, dw_part, m->grid_grad, loss_scale, (const __half*)enc_in,
+                                                 dout, m->mlp_grad_part, m->grid_grad, loss_scale, (const __half*)enc_in,
                                                  (__half*)denc_scratch);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return (int)e;
-  dw_reduce_kernel<<<(W_TOTAL + 255) / 256, 256, 0, st>>>(dw_part, num_sms, m->mlp_grad);
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return (int)e;
+  NSLAM_CHECK_LAUNCH();
+  dw_reduce_kernel<<<(W_TOTAL + 255) / 256, 256, 0, st>>>(m->mlp_grad_part, num_sms, m->mlp_grad);
+  NSLAM_CHECK_LAUNCH();
   if (denc_scratch) {
     // one thread per (sample, level); the sample count lives on the device -> grid-stride over the capacity.
     // Gradients go to a fixed-point accumulator (order-independent sums) and are added to grid_grad afterwards.
-    const size_t n_vals = 2 * (size_t)m->n_grid;
-    long long* acc = (long long*)ngp_scratch(NGP_SCRATCH_GRID, n_vals * sizeof(long long));
-    if (!acc) return (int)cudaErrorMemoryAllocation;
     size_t want = (((size_t)max_samples + 31) / 32 * N_LEVELS * 32 + 255) / 256;
     const size_t cap = (size_t)num_sms * 32;
     grid_scatter_kernel<<<(unsigned)(want < cap ? want : cap), 256, 0, st>>>(coords, counters, (const __half*)denc_scratch, lv,
-                                                                            acc, 1.f / loss_scale);
-    fx_flush_kernel<<<(unsigned)(num_sms * 8), 256, 0, st>>>(acc, m->grid_grad, n_vals, 1.f / GRID_FX);
-    e = cudaGetLastError();
+                                                                            m->grid_grad_fx, 1.f / loss_scale);
+    fx_flush_kernel<<<(unsigned)(num_sms * 8), 256, 0, st>>>(m->grid_grad_fx, m->grid_grad, 2 * (size_t)m->n_grid,
+                                                             1.f / GRID_FX);
+    NSLAM_CHECK_LAUNCH();
   }
-  return (int)e;
+  return 0;
 }
 
 /* one training step with the network on tensor cores: sample -> forward_tc -> loss -> backward_tc
@@ -918,26 +896,18 @@ int nslam_ngp_loss_backward_tc(const nslam_ngp_model* m, const nslam_ngp_batch* 
 int nslam_ngp_density_sample_tc(const nslam_ngp_model* m, const void* packed, int n_per_cascade, unsigned seed,
                                 float decay, int num_sms, void* stream) {
   using namespace ngp;
-  LevelInfo lv;
-  for (int l = 0; l < N_LEVELS; l++) {
-    lv.scale[l] = m->scale[l]; lv.res[l] = m->res[l]; lv.size[l] = m->size[l];
-    lv.offset[l] = m->offset[l]; lv.dense[l] = m->dense[l];
-  }
   const int smem = FwdSmem::TOTAL + 1024;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(density_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return (int)e;
-    configured = true;
-  }
+  if (cudaError_t e = nslam::ensure_dyn_smem<density_tc_kernel>(smem)) return (int)e;
   const int total = n_per_cascade * m->cascades;
   if (total == 0) return 0;
   int grid = (total + 127) / 128;
   if (grid > 4 * num_sms) grid = 4 * num_sms;
-  density_tc_kernel<<<grid, 128, smem, (cudaStream_t)stream>>>((const __half2*)m->grid_half, lv, (const unsigned char*)packed,
-                                                              0.5f - 0.5f * m->aabb_scale, 1.f / m->aabb_scale, m->cascades,
-                                                              n_per_cascade, seed, decay, m->density);
-  return (int)cudaGetLastError();
+  density_tc_kernel<<<grid, 128, smem, (cudaStream_t)stream>>>((const __half2*)m->grid_half, level_info(m),
+                                                              (const unsigned char*)packed, 0.5f - 0.5f * m->aabb_scale,
+                                                              1.f / m->aabb_scale, m->cascades, n_per_cascade, seed, decay,
+                                                              m->density);
+  NSLAM_CHECK_LAUNCH();
+  return 0;
 }
 
 /* NeRF mesh lattice: field / weight [nz,ny,nx] fp32 (DEVICE) of the lattice lo3_host + h (i,j,k) (see mesh_lattice_kernel) */
@@ -945,51 +915,42 @@ int nslam_ngp_mesh_lattice(const nslam_ngp_model* m, const void* packed, const f
                            int nz, float thresh, float* field, float* weight, int num_sms, void* stream) {
   using namespace ngp;
   if (nx <= 0 || ny <= 0 || nz <= 0) return (int)cudaErrorInvalidValue;
-  LevelInfo lv;
-  for (int l = 0; l < N_LEVELS; l++) {
-    lv.scale[l] = m->scale[l]; lv.res[l] = m->res[l]; lv.size[l] = m->size[l];
-    lv.offset[l] = m->offset[l]; lv.dense[l] = m->dense[l];
-  }
   const int smem = FwdSmem::TOTAL + 1024;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(mesh_lattice_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return (int)e;
-    configured = true;
-  }
+  if (cudaError_t e = nslam::ensure_dyn_smem<mesh_lattice_kernel>(smem)) return (int)e;
   const size_t tiles = ((size_t)nx * ny * nz + 127) / 128;
   const int grid = (int)(tiles < (size_t)4 * num_sms ? tiles : (size_t)4 * num_sms);
-  mesh_lattice_kernel<<<grid, 128, smem, (cudaStream_t)stream>>>((const __half2*)m->grid_half, lv, (const unsigned char*)packed,
-                                                                 0.5f - 0.5f * m->aabb_scale, 1.f / m->aabb_scale, m->cascades,
-                                                                 m->density, make_float3(lo3_host[0], lo3_host[1], lo3_host[2]),
+  mesh_lattice_kernel<<<grid, 128, smem, (cudaStream_t)stream>>>((const __half2*)m->grid_half, level_info(m),
+                                                                 (const unsigned char*)packed, 0.5f - 0.5f * m->aabb_scale,
+                                                                 1.f / m->aabb_scale, m->cascades, m->density,
+                                                                 make_float3(lo3_host[0], lo3_host[1], lo3_host[2]),
                                                                  h, nx, ny, nz, thresh, field, weight);
-  return (int)cudaGetLastError();
+  NSLAM_CHECK_LAUNCH();
+  return 0;
 }
 
 /* NeRF mesh vertex colours: colors [n,3] = network radiance at vertices [n,3] seen along -normals [n,3] (DEVICE), through
- * the tensor-core forward in chunks of library-owned scratch; srgb != 0: encoded with the inverse of the ingest's curve */
+ * the tensor-core forward in chunks of 2^18 vertices; srgb != 0: encoded with the inverse of the ingest's curve.
+ * scratch: one chunk's network outputs [cap,4] followed by its input records [cap,7], fp32, cap = min(n, 2^18) */
 int nslam_ngp_mesh_colors(const nslam_ngp_model* m, const void* packed, const float* vertices, const float* normals, int n,
-                          int srgb, float* colors, int num_sms, void* stream) {
+                          int srgb, float* colors, void* scratch, long long scratch_bytes, int num_sms, void* stream) {
   using namespace ngp;
   if (n < 0) return (int)cudaErrorInvalidValue;
   if (n == 0) return 0;
   constexpr int CHUNK = 1 << 18;
   const int cap = n < CHUNK ? n : CHUNK;
-  float* rgbsigma = (float*)ngp_scratch(NGP_SCRATCH_MESH, (size_t)cap * 11 * sizeof(float));   // [cap,4] then [cap,7]
-  if (!rgbsigma) return (int)cudaErrorMemoryAllocation;
+  if (scratch_bytes < 44LL * cap) return (int)cudaErrorInvalidValue;
+  float* rgbsigma = (float*)scratch;
   float* coords = rgbsigma + (size_t)cap * 4;
   cudaStream_t st = (cudaStream_t)stream;
   for (int base = 0; base < n; base += CHUNK) {
     const int c = n - base < CHUNK ? n - base : CHUNK;
     mesh_color_records_kernel<<<(c + 255) / 256, 256, 0, st>>>(vertices + 3 * (size_t)base, normals + 3 * (size_t)base, c,
                                                                0.5f - 0.5f * m->aabb_scale, 1.f / m->aabb_scale, coords);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return (int)e;
+    NSLAM_CHECK_LAUNCH();
     int r = nslam_ngp_forward_tc(m, packed, coords, nullptr, c, c, rgbsigma, nullptr, num_sms, stream);
     if (r) return r;
     mesh_color_store_kernel<<<(c + 255) / 256, 256, 0, st>>>((const float4*)rgbsigma, c, srgb, colors + 3 * (size_t)base);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return (int)e;
+    NSLAM_CHECK_LAUNCH();
   }
   return 0;
 }

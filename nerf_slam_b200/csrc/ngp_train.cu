@@ -23,13 +23,6 @@
 //   ngp_adam           fused Adam (+L2 on the MLP, zero-gradient skip on hash entries) writing
 //                      the fp32 master and the fp16 compute copy
 #include "ngp_common.cuh"
-#include "../../include/nslam_ngp.h"
-
-#define NGP_CHECK_LAUNCH()                        \
-  do {                                            \
-    cudaError_t e__ = cudaGetLastError();         \
-    if (e__ != cudaSuccess) return (int)e__;      \
-  } while (0)
 
 namespace ngp {
 
@@ -877,14 +870,6 @@ __global__ void ingest_batch_kernel(const uint8_t* __restrict__ rgb_chw, const f
 
 // ============================================================================================
 namespace ngp {
-static LevelInfo make_lv(const nslam_ngp_model* m) {
-  LevelInfo lv;
-  for (int l = 0; l < N_LEVELS; l++) {
-    lv.scale[l] = m->scale[l]; lv.res[l] = m->res[l]; lv.size[l] = m->size[l];
-    lv.offset[l] = m->offset[l]; lv.dense[l] = m->dense[l];
-  }
-  return lv;
-}
 static Scene make_scene(const nslam_ngp_model* m) {
   Scene s;
   s.aabb_lo = 0.5f - 0.5f * m->aabb_scale; s.aabb_hi = 0.5f + 0.5f * m->aabb_scale;
@@ -900,16 +885,9 @@ static ImageStore make_store(const nslam_ngp_images* im) {
 constexpr size_t FWD_SMEM = (W_TOTAL + 64 * LD) * sizeof(float);
 constexpr size_t BWD_SMEM = (W_TOTAL + (64 + 64) * LD) * sizeof(float) + 256 * LD * sizeof(__half);
 static int ensure_attrs() {
-  static bool done = false;
-  if (done) return 0;
-  cudaError_t e = cudaFuncSetAttribute(forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FWD_SMEM);
-  if (e != cudaSuccess) return (int)e;
-  e = cudaFuncSetAttribute(backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM);
-  if (e != cudaSuccess) return (int)e;
-  e = cudaFuncSetAttribute(density_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FWD_SMEM);
-  if (e != cudaSuccess) return (int)e;
-  done = true;
-  return 0;
+  if (cudaError_t e = nslam::ensure_dyn_smem<forward_kernel>(FWD_SMEM)) return (int)e;
+  if (cudaError_t e = nslam::ensure_dyn_smem<backward_kernel>(BWD_SMEM)) return (int)e;
+  return (int)nslam::ensure_dyn_smem<density_sample_kernel>(FWD_SMEM);
 }
 }  // namespace ngp
 
@@ -937,23 +915,21 @@ int nslam_ngp_train_step(const nslam_ngp_model* m, const nslam_ngp_images* im, c
   if (n_rays > b->max_rays) return (int)cudaErrorInvalidValue;
   cudaMemsetAsync(b->counters, 0, 4 * sizeof(int), st);
   cudaMemsetAsync(b->loss, 0, sizeof(float), st);
-  const LevelInfo lv = make_lv(m);
+  const LevelInfo lv = level_info(m);
   const Scene sc = make_scene(m);
   sample_rays(m, im, b, n_rays, seed, st);
-  NGP_CHECK_LAUNCH();
+  NSLAM_CHECK_LAUNCH();
   forward_kernel<<<(b->max_samples + TILE - 1) / TILE, TILE, FWD_SMEM, st>>>(
       b->coords, b->counters, -1, (const __half2*)m->grid_half, lv, m->mlp, b->rgbsigma);
-  NGP_CHECK_LAUNCH();
-  long long* loss_fx = (long long*)ngp_scratch(NGP_SCRATCH_LOSS, sizeof(long long));
-  if (!loss_fx) return (int)cudaErrorMemoryAllocation;
+  NSLAM_CHECK_LAUNCH();
   loss_kernel<<<(n_rays + 3) / 4, 128, 0, st>>>(b->rays, n_rays, b->coords, b->tdist, b->rgbsigma,
                                                      b->counters, lambda_depth, make_float3(bg_r, bg_g, bg_b),
-                                                     0, b->dout, b->loss, nullptr, loss_fx);
-  fx_flush_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(loss_fx, b->loss, 1, 1.f / LOSS_FX);
-  NGP_CHECK_LAUNCH();
+                                                     0, b->dout, b->loss, nullptr, b->loss_fx);
+  fx_flush_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(b->loss_fx, b->loss, 1, 1.f / LOSS_FX);
+  NSLAM_CHECK_LAUNCH();
   backward_kernel<<<2 * num_sms, TILE, BWD_SMEM, st>>>(b->coords, b->counters, (const __half2*)m->grid_half,
                                                        lv, m->mlp, b->dout, m->mlp_grad, m->grid_grad);
-  NGP_CHECK_LAUNCH();
+  NSLAM_CHECK_LAUNCH();
   return 0;
 }
 
@@ -967,20 +943,18 @@ int nslam_ngp_sample_phase(const nslam_ngp_model* m, const nslam_ngp_images* im,
   cudaMemsetAsync(b->counters, 0, 4 * sizeof(int), st);
   cudaMemsetAsync(b->loss, 0, sizeof(float), st);
   sample_rays(m, im, b, n_rays, seed, st);
-  NGP_CHECK_LAUNCH();
+  NSLAM_CHECK_LAUNCH();
   return 0;
 }
 
 int nslam_ngp_loss_phase(const nslam_ngp_batch* b, int n_rays, float lambda_depth, float bg_r, float bg_g,
                          float bg_b, void* stream) {
   using namespace ngp;
-  long long* loss_fx = (long long*)ngp_scratch(NGP_SCRATCH_LOSS, sizeof(long long));
-  if (!loss_fx) return (int)cudaErrorMemoryAllocation;
   loss_kernel<<<(n_rays + 3) / 4, 128, 0, (cudaStream_t)stream>>>(b->rays, n_rays, b->coords, b->tdist, b->rgbsigma,
                                                                        b->counters, lambda_depth,
-                                                                       make_float3(bg_r, bg_g, bg_b), 0, b->dout, b->loss, nullptr, loss_fx);
-  fx_flush_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(loss_fx, b->loss, 1, 1.f / LOSS_FX);
-  NGP_CHECK_LAUNCH();
+                                                                       make_float3(bg_r, bg_g, bg_b), 0, b->dout, b->loss, nullptr, b->loss_fx);
+  fx_flush_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(b->loss_fx, b->loss, 1, 1.f / LOSS_FX);
+  NSLAM_CHECK_LAUNCH();
   return 0;
 }
 
@@ -993,11 +967,11 @@ int nslam_ngp_adam(const nslam_ngp_model* m, int step, float lr, float beta1, fl
   adam_kernel<<<(unsigned)((ng4 + 255) / 256), 256, 0, st>>>((float4*)m->grid_master, (float4*)m->grid_grad, (float4*)m->grid_m,
                                                             (float4*)m->grid_v, (__half2*)m->grid_half, ng4, lr, beta1, beta2,
                                                             eps, 0.f, 1, bc1, bc2);
-  NGP_CHECK_LAUNCH();
+  NSLAM_CHECK_LAUNCH();
   adam_kernel<<<(W_TOTAL / 4 + 255) / 256, 256, 0, st>>>((float4*)m->mlp, (float4*)m->mlp_grad, (float4*)m->mlp_m,
                                                          (float4*)m->mlp_v, nullptr, W_TOTAL / 4, lr, beta1, beta2, eps,
                                                          l2_mlp, 0, bc1, bc2);
-  NGP_CHECK_LAUNCH();
+  NSLAM_CHECK_LAUNCH();
   return 0;
 }
 
@@ -1008,8 +982,8 @@ int nslam_ngp_forward(const nslam_ngp_model* m, const float* coords, int n, floa
   if (r) return r;
   if (n == 0) return 0;
   forward_kernel<<<(n + TILE - 1) / TILE, TILE, FWD_SMEM, (cudaStream_t)stream>>>(
-      coords, nullptr, n, (const __half2*)m->grid_half, make_lv(m), m->mlp, rgbsigma);
-  NGP_CHECK_LAUNCH();
+      coords, nullptr, n, (const __half2*)m->grid_half, level_info(m), m->mlp, rgbsigma);
+  NSLAM_CHECK_LAUNCH();
   return 0;
 }
 
@@ -1023,19 +997,17 @@ int nslam_ngp_loss_backward(const nslam_ngp_model* m, const nslam_ngp_batch* b, 
   int h[4] = {n_samples, n_rays, n_rays, 0};
   cudaMemcpyAsync(b->counters, h, sizeof(h), cudaMemcpyHostToDevice, st);
   cudaMemsetAsync(b->loss, 0, sizeof(float), st);
-  const LevelInfo lv = make_lv(m);
+  const LevelInfo lv = level_info(m);
   forward_kernel<<<(n_samples + TILE - 1) / TILE, TILE, FWD_SMEM, st>>>(b->coords, b->counters, -1,
                                                                        (const __half2*)m->grid_half, lv, m->mlp, b->rgbsigma);
-  NGP_CHECK_LAUNCH();
-  long long* loss_fx = (long long*)ngp_scratch(NGP_SCRATCH_LOSS, sizeof(long long));
-  if (!loss_fx) return (int)cudaErrorMemoryAllocation;
+  NSLAM_CHECK_LAUNCH();
   loss_kernel<<<(n_rays + 3) / 4, 128, 0, st>>>(b->rays, n_rays, b->coords, b->tdist, b->rgbsigma, b->counters,
-                                                     lambda_depth, make_float3(bg_r, bg_g, bg_b), 0, b->dout, b->loss, nullptr, loss_fx);
-  fx_flush_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(loss_fx, b->loss, 1, 1.f / LOSS_FX);
-  NGP_CHECK_LAUNCH();
+                                                     lambda_depth, make_float3(bg_r, bg_g, bg_b), 0, b->dout, b->loss, nullptr, b->loss_fx);
+  fx_flush_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(b->loss_fx, b->loss, 1, 1.f / LOSS_FX);
+  NSLAM_CHECK_LAUNCH();
   backward_kernel<<<2 * num_sms, TILE, BWD_SMEM, st>>>(b->coords, b->counters, (const __half2*)m->grid_half, lv,
                                                        m->mlp, b->dout, m->mlp_grad, m->grid_grad);
-  NGP_CHECK_LAUNCH();
+  NSLAM_CHECK_LAUNCH();
   return 0;
 }
 
@@ -1051,22 +1023,22 @@ int nslam_ngp_update_density_grid(const nslam_ngp_model* m, const nslam_ngp_imag
   const size_t total = NC * m->cascades;
   density_mark_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const Camera*)im->cams, im->active,
                                                                       im->n_active, m->cascades, m->density);
-  NGP_CHECK_LAUNCH();
+  NSLAM_CHECK_LAUNCH();
   const int n = n_per_cascade * m->cascades;
   if (packed) {
     r = nslam_ngp_density_sample_tc(m, packed, n_per_cascade, seed, decay, num_sms, stream);
     if (r) return r;
   } else {
-    density_sample_kernel<<<(n + TILE - 1) / TILE, TILE, FWD_SMEM, st>>>((const __half2*)m->grid_half, make_lv(m), m->mlp,
+    density_sample_kernel<<<(n + TILE - 1) / TILE, TILE, FWD_SMEM, st>>>((const __half2*)m->grid_half, level_info(m), m->mlp,
                                                                        make_scene(m), n_per_cascade, seed, decay, m->density);
-    NGP_CHECK_LAUNCH();
+    NSLAM_CHECK_LAUNCH();
   }
   density_mean_kernel<<<DM_BLOCKS, 256, 0, st>>>(m->density, total);
   density_mean_final_kernel<<<1, 32, 0, st>>>(m->stats);
-  NGP_CHECK_LAUNCH();
+  NSLAM_CHECK_LAUNCH();
   density_bits_kernel<<<(unsigned)((total / 8 + 255) / 256), 256, 0, st>>>(m->density, total / 8, m->stats,
                                                                           min_thickness, m->bits);
-  NGP_CHECK_LAUNCH();
+  NSLAM_CHECK_LAUNCH();
   return 0;
 }
 
@@ -1085,21 +1057,21 @@ int nslam_ngp_render_tile(const nslam_ngp_model* m, const nslam_ngp_batch* b, co
   cam.fx = cam16[12]; cam.fy = cam16[13]; cam.cx = cam16[14]; cam.cy = cam16[15];
   cam.w = (int)cam16[16]; cam.h = (int)cam16[17];
   cudaMemsetAsync(b->counters, 0, 4 * sizeof(int), st);
-  const LevelInfo lv = make_lv(m);
+  const LevelInfo lv = level_info(m);
   render_rays_kernel<<<(tw * th + 3) / 4, 128, 0, st>>>(cam, make_scene(m), m->bits, x0, y0, tw, th,
                                                            b->max_samples, max_per_ray, b->rays, b->coords, b->tdist, b->counters);
-  NGP_CHECK_LAUNCH();
+  NSLAM_CHECK_LAUNCH();
   if (packed) {
     r = nslam_ngp_forward_tc(m, packed, b->coords, b->counters, -1, b->max_samples, b->rgbsigma, nullptr, num_sms, stream);
     if (r) return r;
   } else {
     forward_kernel<<<(b->max_samples + TILE - 1) / TILE, TILE, FWD_SMEM, st>>>(b->coords, b->counters, -1,
                                                                               (const __half2*)m->grid_half, lv, m->mlp, b->rgbsigma);
-    NGP_CHECK_LAUNCH();
+    NSLAM_CHECK_LAUNCH();
   }
   loss_kernel<<<(tw * th + 3) / 4, 128, 0, st>>>(b->rays, tw * th, b->coords, b->tdist, b->rgbsigma, b->counters,
                                                       0.f, make_float3(bg_r, bg_g, bg_b), 1, nullptr, nullptr, out_rgbd);
-  NGP_CHECK_LAUNCH();
+  NSLAM_CHECK_LAUNCH();
   return 0;
 }
 
@@ -1108,7 +1080,7 @@ int nslam_ngp_ingest_image(const unsigned char* rgb_chw, const float* idepth_up,
                            int H, int W, void* rgba_slot, float* depth_slot, float* cov_slot, void* stream) {
   ngp::ingest_image_kernel<<<(H * W + 255) / 256, 256, 0, (cudaStream_t)stream>>>(
       rgb_chw, idepth_up, depth_cov_up, H, W, (__half*)rgba_slot, depth_slot, cov_slot);
-  NGP_CHECK_LAUNCH();
+  NSLAM_CHECK_LAUNCH();
   return 0;
 }
 
@@ -1126,7 +1098,7 @@ int nslam_ngp_ingest_batch(const unsigned char* rgb_chw, const float* idepth_up,
   ngp::ingest_batch_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
       rgb_chw, idepth_up, depth_cov_up, ids, H, W, (__half*)rgba, depth, depth_cov, cam_T_world, fx, fy, cx, cy,
       (ngp::Camera*)cams, (ngp::Camera*)cams_base, cam_state, cam_steps, n_slots);
-  NGP_CHECK_LAUNCH();
+  NSLAM_CHECK_LAUNCH();
   return 0;
 }
 

@@ -188,8 +188,6 @@ __global__ void __launch_bounds__(256) pc_voxel_reduce_kernel(const float* point
   out_counts[r] = e - s;
 }
 
-static size_t pc_align(size_t x) { return (x + 255) & ~(size_t)255; }
-
 static bool pc_shape_ok(int n, int H, int W) { return n > 0 && H > 0 && W > 0 && (long long)n * H * W <= INT_MAX; }
 
 // cloud scratch: counts, offsets [nblk + 1] int; CUB scan storage
@@ -206,15 +204,13 @@ static size_t cloud_scratch(int n, int H, int W, void* base, CloudScratch* s) {
   t.nblk = n * t.bpf;
   size_t scan_bytes = 0;
   cub::DeviceScan::ExclusiveSum((void*)nullptr, scan_bytes, (const int*)nullptr, (int*)nullptr, t.nblk + 1);
-  size_t off = 0;
-  char* b = (char*)base;
-  auto take = [&](size_t bytes) { void* p = b ? b + off : nullptr; off += pc_align(bytes); return p; };
-  t.counts = (int*)take(4 * ((size_t)t.nblk + 1));
-  t.offsets = (int*)take(4 * ((size_t)t.nblk + 1));
+  ScratchCarver c(base);
+  t.counts = c.take<int>(4 * ((size_t)t.nblk + 1));
+  t.offsets = c.take<int>(4 * ((size_t)t.nblk + 1));
   t.cub_bytes = scan_bytes;
-  t.cub = take(scan_bytes);
+  t.cub = c.take(scan_bytes);
   if (s) *s = t;
-  return off;
+  return c.off;
 }
 
 // downsampling scratch: keys, sorted keys [N] u64; index, order, head, rank [N] int; starts [N + 1] int; CUB storage
@@ -230,21 +226,19 @@ static size_t voxel_scratch(int N, void* base, VoxelScratch* s) {
   cub::DeviceRadixSort::SortPairs((void*)nullptr, sort_bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
                                   (const int*)nullptr, (int*)nullptr, N);
   cub::DeviceScan::ExclusiveSum((void*)nullptr, scan_bytes, (const int*)nullptr, (int*)nullptr, N);
-  size_t off = 0;
-  char* b = (char*)base;
-  auto take = [&](size_t bytes) { void* p = b ? b + off : nullptr; off += pc_align(bytes); return p; };
+  ScratchCarver c(base);
   VoxelScratch t;
-  t.keys = (unsigned long long*)take(8 * (size_t)N);
-  t.sorted = (unsigned long long*)take(8 * (size_t)N);
-  t.index = (int*)take(4 * (size_t)N);
-  t.order = (int*)take(4 * (size_t)N);
-  t.head = (int*)take(4 * (size_t)N);
-  t.rank = (int*)take(4 * (size_t)N);
-  t.starts = (int*)take(4 * ((size_t)N + 1));
+  t.keys = c.take<unsigned long long>(8 * (size_t)N);
+  t.sorted = c.take<unsigned long long>(8 * (size_t)N);
+  t.index = c.take<int>(4 * (size_t)N);
+  t.order = c.take<int>(4 * (size_t)N);
+  t.head = c.take<int>(4 * (size_t)N);
+  t.rank = c.take<int>(4 * (size_t)N);
+  t.starts = c.take<int>(4 * ((size_t)N + 1));
   t.cub_bytes = sort_bytes > scan_bytes ? sort_bytes : scan_bytes;
-  t.cub = take(t.cub_bytes);
+  t.cub = c.take(t.cub_bytes);
   if (s) *s = t;
-  return off;
+  return c.off;
 }
 
 static CloudArgs cloud_args(const float* pose, const float* idepth, const float* cov, const float* views, int min_views,

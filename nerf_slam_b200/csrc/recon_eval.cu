@@ -123,8 +123,6 @@ __global__ void __launch_bounds__(256) ev_sample_kernel(const float* V, const in
   if (tri) tri[i] = lo;
 }
 
-static size_t ev_align(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct SurfaceScratch {
   unsigned long long *w, *cdf;
   void* cub;
@@ -134,16 +132,14 @@ struct SurfaceScratch {
 static size_t surface_scratch(int nt, void* base, SurfaceScratch* s) {
   size_t scan_bytes = 0;
   cub::DeviceScan::InclusiveSum((void*)nullptr, scan_bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, nt);
-  size_t off = 0;
-  char* b = (char*)base;
-  auto take = [&](size_t bytes) { void* p = b ? b + off : nullptr; off += ev_align(bytes); return p; };
+  ScratchCarver c(base);
   SurfaceScratch t;
-  t.w = (unsigned long long*)take(8 * (size_t)nt);
-  t.cdf = (unsigned long long*)take(8 * (size_t)nt);
+  t.w = c.take<unsigned long long>(8 * (size_t)nt);
+  t.cdf = c.take<unsigned long long>(8 * (size_t)nt);
   t.cub_bytes = scan_bytes;
-  t.cub = take(scan_bytes);
+  t.cub = c.take(scan_bytes);
   if (s) *s = t;
-  return off;
+  return c.off;
 }
 
 // ----------------------------------------------------------------------------------------------------------------- BVH
@@ -315,23 +311,21 @@ static size_t bvh_layout(int n, int B, void* base, BvhLayout* s) {
   size_t sort_bytes = 0;
   cub::DeviceRadixSort::SortPairs((void*)nullptr, sort_bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
                                   (const int*)nullptr, (int*)nullptr, n);
-  size_t off = 0;
-  char* b = (char*)base;
-  auto take = [&](size_t bytes) { void* p = b ? b + off : nullptr; off += ev_align(bytes); return p; };
-  t.bounds = (unsigned*)take(6 * 4);
-  t.keys = (unsigned long long*)take(8 * (size_t)n);
-  t.sorted = (unsigned long long*)take(8 * (size_t)n);
-  t.index = (int*)take(4 * (size_t)n);
-  t.order = (int*)take(4 * (size_t)n);
-  t.pts = (float4*)take(16 * (size_t)n);
-  t.box = (float*)take(24 * nodes);
-  t.child = (int2*)take(8 * (size_t)t.L);
-  t.parent = (int*)take(4 * nodes);
-  t.flags = (int*)take(4 * (size_t)t.L);
+  ScratchCarver c(base);
+  t.bounds = c.take<unsigned>(6 * 4);
+  t.keys = c.take<unsigned long long>(8 * (size_t)n);
+  t.sorted = c.take<unsigned long long>(8 * (size_t)n);
+  t.index = c.take<int>(4 * (size_t)n);
+  t.order = c.take<int>(4 * (size_t)n);
+  t.pts = c.take<float4>(16 * (size_t)n);
+  t.box = c.take<float>(24 * nodes);
+  t.child = c.take<int2>(8 * (size_t)t.L);
+  t.parent = c.take<int>(4 * nodes);
+  t.flags = c.take<int>(4 * (size_t)t.L);
   t.cub_bytes = sort_bytes;
-  t.cub = take(sort_bytes);
+  t.cub = c.take(sort_bytes);
   if (s) *s = t;
-  return off;
+  return c.off;
 }
 
 struct QueryScratch {
@@ -345,18 +339,16 @@ static size_t query_scratch(int n, void* base, QueryScratch* s) {
   size_t sort_bytes = 0;
   cub::DeviceRadixSort::SortPairs((void*)nullptr, sort_bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
                                   (const int*)nullptr, (int*)nullptr, n);
-  size_t off = 0;
-  char* b = (char*)base;
-  auto take = [&](size_t bytes) { void* p = b ? b + off : nullptr; off += ev_align(bytes); return p; };
+  ScratchCarver c(base);
   QueryScratch t;
-  t.keys = (unsigned long long*)take(8 * (size_t)n);
-  t.sorted = (unsigned long long*)take(8 * (size_t)n);
-  t.index = (int*)take(4 * (size_t)n);
-  t.order = (int*)take(4 * (size_t)n);
+  t.keys = c.take<unsigned long long>(8 * (size_t)n);
+  t.sorted = c.take<unsigned long long>(8 * (size_t)n);
+  t.index = c.take<int>(4 * (size_t)n);
+  t.order = c.take<int>(4 * (size_t)n);
   t.cub_bytes = sort_bytes;
-  t.cub = take(sort_bytes);
+  t.cub = c.take(sort_bytes);
   if (s) *s = t;
-  return off;
+  return c.off;
 }
 
 // fp64 squared distance of q to a box with the points' rounded operations: per axis the gap max(lo - q, q - hi, 0)

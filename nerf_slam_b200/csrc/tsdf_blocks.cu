@@ -310,28 +310,24 @@ struct ActScratch {
   size_t cub_bytes;
 };
 
-static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 static size_t act_scratch(int n, void* base, ActScratch* s) {
   size_t sort_bytes = 0, scan_bytes = 0;
   cub::DeviceRadixSort::SortKeys((void*)nullptr, sort_bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, n);
   cub::DeviceScan::ExclusiveSum((void*)nullptr, scan_bytes, (const int*)nullptr, (int*)nullptr, n);
   const size_t cub_bytes = sort_bytes > scan_bytes ? sort_bytes : scan_bytes;
-  size_t off = 0;
-  char* b = (char*)base;
-  auto take = [&](size_t bytes) { void* p = b ? b + off : nullptr; off += align256(bytes); return p; };
+  ScratchCarver c(base);
   ActScratch t;
-  t.keys = (unsigned long long*)take(8 * (size_t)n);
-  t.sorted = (unsigned long long*)take(8 * (size_t)n);
-  t.is_new = (int*)take(4 * (size_t)n);
-  t.new_rank = (int*)take(4 * (size_t)n);
-  t.pool = (int*)take(4 * (size_t)n);
-  t.head = (int*)take(4 * (size_t)n);
-  t.head_rank = (int*)take(4 * (size_t)n);
+  t.keys = c.take<unsigned long long>(8 * (size_t)n);
+  t.sorted = c.take<unsigned long long>(8 * (size_t)n);
+  t.is_new = c.take<int>(4 * (size_t)n);
+  t.new_rank = c.take<int>(4 * (size_t)n);
+  t.pool = c.take<int>(4 * (size_t)n);
+  t.head = c.take<int>(4 * (size_t)n);
+  t.head_rank = c.take<int>(4 * (size_t)n);
   t.cub_bytes = cub_bytes;
-  t.cub = take(cub_bytes);
+  t.cub = c.take(cub_bytes);
   if (s) *s = t;
-  return off;
+  return c.off;
 }
 
 }  // namespace nslam

@@ -100,12 +100,7 @@ static int launch_upsample(const float* data, const float* data2, const void* ma
                            const long long* index, int K, int ht, int wd, float pw, cudaStream_t st) {
   dim3 grid((wd + UX - 1) / UX, ht, K);
   const size_t smem = (NHWC ? (size_t)UX * UROW : (size_t)576 * UX) * sizeof(T);
-  static bool configured = false;
-  if (!configured && smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(cvx_upsample_kernel<T, NHWC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return (int)e;
-    configured = true;
-  }
+  if (cudaError_t e = ensure_dyn_smem<cvx_upsample_kernel<T, NHWC>>(smem)) return (int)e;
   cvx_upsample_kernel<T, NHWC><<<grid, 256, smem, st>>>(data, data2, (const T*)mask, out, out2, index, ht, wd, pw);
   NSLAM_CHECK_LAUNCH();
   return 0;

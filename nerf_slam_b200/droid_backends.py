@@ -188,14 +188,12 @@ def altcorr_backward(fmap1, fmap2, coords, corr_grad, radius):
     if (fmap2.shape[0] != B or fmap2.shape[3] != C or tuple(coords.shape) != (B, N, H1, W1, 2)
             or tuple(corr_grad.shape) != (B, N, rd * rd, H1, W1)):
         raise RuntimeError("altcorr_backward: shape mismatch")
-    nbytes = ctypes.c_ulonglong(0)
-    _lib.check(lib.nslam_altcorr_backward_scratch(B, N, H1, W1, H2, W2, C, radius, ctypes.byref(nbytes)),
-               "altcorr_backward (unsupported shape)")
-    scratch = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=fmap1.device)
+    nbytes = _lib.query_size("nslam_altcorr_backward_scratch", B, N, H1, W1, H2, W2, C, radius)
+    scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=fmap1.device)
     g1 = torch.empty_like(fmap1)
     g2 = torch.empty_like(fmap2)
     _lib.check(lib.nslam_altcorr_backward(_lib.ptr(fmap1), _lib.ptr(fmap2), _lib.ptr(coords), _lib.ptr(corr_grad),
-                                          _lib.ptr(g1), _lib.ptr(g2), _lib.ptr(scratch), nbytes.value, B, N, H1, W1,
+                                          _lib.ptr(g1), _lib.ptr(g2), _lib.ptr(scratch), nbytes, B, N, H1, W1,
                                           H2, W2, C, radius, _lib.stream_ptr()), "altcorr_backward")
     return [g1, g2, torch.zeros_like(coords)]
 

@@ -74,14 +74,12 @@ def sample_surface(mesh, n, seed=0, return_triangles=False):
     if nt == 0 or nv == 0:
         raise ValueError("the mesh has no triangle")
     dev = V.device
-    nb = np.zeros(1, np.int64)
-    _lib.check(lib.nslam_eval_surface_scratch(nt, nb.ctypes.data), "eval_surface_scratch")
-    scratch = torch.empty(int(nb[0]), dtype=torch.uint8, device=dev)
+    scratch = torch.empty(_lib.query_size("nslam_eval_surface_scratch", nt), dtype=torch.uint8, device=dev)
     info = torch.empty(2, dtype=torch.int64, device=dev)
     points = torch.empty(n, 3, dtype=torch.float32, device=dev)
     tri = torch.empty(n, dtype=torch.int32, device=dev) if return_triangles else None
     with _lib.fixed_stream():
-        _lib.check(lib.nslam_eval_surface_area(_lib.ptr(V), nv, _lib.ptr(T), nt, _lib.ptr(scratch), int(nb[0]),
+        _lib.check(lib.nslam_eval_surface_area(_lib.ptr(V), nv, _lib.ptr(T), nt, _lib.ptr(scratch), scratch.numel(),
                                                _lib.ptr(info), _lib.stream_ptr()), "eval_surface_area")
         total, flags = info.tolist()
         if flags & 1:
@@ -94,7 +92,7 @@ def sample_surface(mesh, n, seed=0, return_triangles=False):
             raise ValueError("the mesh has no area to sample")
         if n:
             _lib.check(lib.nslam_eval_sample_surface(_lib.ptr(V), _lib.ptr(T), nt, n, int(seed) % (1 << 64),
-                                                     _lib.ptr(scratch), int(nb[0]), _lib.ptr(points), _lib.ptr(tri),
+                                                     _lib.ptr(scratch), scratch.numel(), _lib.ptr(points), _lib.ptr(tri),
                                                      _lib.stream_ptr()), "eval_sample_surface")
     return (points, tri) if return_triangles else points
 
@@ -111,10 +109,9 @@ class PointIndex:
             raise ValueError("the reference has no point")
         if not 1 <= self.leaf_size <= 32:
             raise ValueError(f"leaf_size must be in 1..32, got {leaf_size}")
-        nb = np.zeros(1, np.int64)
-        _lib.check(lib.nslam_eval_bvh_scratch(self.n, self.leaf_size, nb.ctypes.data), "eval_bvh_scratch")
-        self.bvh = torch.empty(int(nb[0]), dtype=torch.uint8, device=self.device)
-        _lib.check(lib.nslam_eval_bvh_build(_lib.ptr(ref), self.n, self.leaf_size, _lib.ptr(self.bvh), int(nb[0]),
+        self.bvh = torch.empty(_lib.query_size("nslam_eval_bvh_scratch", self.n, self.leaf_size), dtype=torch.uint8,
+                               device=self.device)
+        _lib.check(lib.nslam_eval_bvh_build(_lib.ptr(ref), self.n, self.leaf_size, _lib.ptr(self.bvh), self.bvh.numel(),
                                             _lib.stream_ptr()), "eval_bvh_build")
 
     def query(self, query, max_dist=math.inf, num_sms=0):
@@ -132,11 +129,9 @@ class PointIndex:
         idx = torch.empty(m, dtype=torch.int64, device=self.device)
         if m == 0:
             return dist, idx
-        nb = np.zeros(1, np.int64)
-        _lib.check(lib.nslam_eval_nearest_scratch(m, nb.ctypes.data), "eval_nearest_scratch")
-        scratch = torch.empty(int(nb[0]), dtype=torch.uint8, device=self.device)
+        scratch = torch.empty(_lib.query_size("nslam_eval_nearest_scratch", m), dtype=torch.uint8, device=self.device)
         _lib.check(lib.nslam_eval_nearest(_lib.ptr(self.bvh), self.bvh.numel(), self.n, self.leaf_size, _lib.ptr(q), m,
-                                          float(max_dist), int(num_sms), _lib.ptr(scratch), int(nb[0]), _lib.ptr(dist),
+                                          float(max_dist), int(num_sms), _lib.ptr(scratch), scratch.numel(), _lib.ptr(dist),
                                           _lib.ptr(idx), _lib.stream_ptr()), "eval_nearest")
         return dist, idx
 

@@ -87,14 +87,12 @@ class _CloudKernels:
         lib = _lib.load()
         n, H, W = idepths.shape
         dev = idepths.device
-        nb = np.zeros(1, np.int64)
-        _lib.check(lib.nslam_point_cloud_scratch(n, H, W, nb.ctypes.data), "point_cloud_scratch")
-        scratch = torch.empty(int(nb[0]), dtype=torch.uint8, device=dev)
+        scratch = torch.empty(_lib.query_size("nslam_point_cloud_scratch", n, H, W), dtype=torch.uint8, device=dev)
         total = torch.empty(1, dtype=torch.int32, device=dev)
         mv = int(min_views) if views is not None else 0
         with _lib.fixed_stream():
             _lib.check(lib.nslam_point_cloud_count(_lib.ptr(idepths), _lib.ptr(covs), _lib.ptr(views), mv, n, H, W,
-                                                   float(max_depth), float(max_sigma), _lib.ptr(scratch), int(nb[0]),
+                                                   float(max_depth), float(max_sigma), _lib.ptr(scratch), scratch.numel(),
                                                    _lib.ptr(total), _lib.stream_ptr()), "point_cloud_count")
             N = int(total.item())
             points = torch.empty(N, 3, dtype=torch.float32, device=dev)
@@ -102,7 +100,7 @@ class _CloudKernels:
             if N:
                 _lib.check(lib.nslam_point_cloud_emit(
                     _lib.ptr(poses), _lib.ptr(idepths), _lib.ptr(covs), _lib.ptr(views), mv, _lib.ptr(images), _lib.ptr(intr),
-                    n, H, W, float(max_depth), float(max_sigma), _lib.ptr(scratch), int(nb[0]), _lib.ptr(points),
+                    n, H, W, float(max_depth), float(max_sigma), _lib.ptr(scratch), scratch.numel(), _lib.ptr(points),
                     _lib.ptr(colors), _lib.stream_ptr()), "point_cloud_emit")
         return points, colors
 
@@ -113,18 +111,16 @@ class _CloudKernels:
         lib = _lib.load()
         N = int(points.shape[0])
         dev = points.device
-        nb = np.zeros(1, np.int64)
-        _lib.check(lib.nslam_point_cloud_voxel_scratch(N, nb.ctypes.data), "point_cloud_voxel_scratch")
-        scratch = torch.empty(int(nb[0]), dtype=torch.uint8, device=dev)
+        scratch = torch.empty(_lib.query_size("nslam_point_cloud_voxel_scratch", N), dtype=torch.uint8, device=dev)
         nv = torch.empty(1, dtype=torch.int32, device=dev)
         with _lib.fixed_stream():
-            _lib.check(lib.nslam_point_cloud_voxel_sort(_lib.ptr(points), N, float(voxel_size), _lib.ptr(scratch), int(nb[0]),
+            _lib.check(lib.nslam_point_cloud_voxel_sort(_lib.ptr(points), N, float(voxel_size), _lib.ptr(scratch), scratch.numel(),
                                                         _lib.ptr(nv), _lib.stream_ptr()), "point_cloud_voxel_sort")
             V = int(nv.item())
             out_p = torch.empty(V, 3, dtype=torch.float32, device=dev)
             out_c = torch.empty(V, 3, dtype=torch.float32, device=dev)
             out_n = torch.empty(V, dtype=torch.int32, device=dev)
-            _lib.check(lib.nslam_point_cloud_voxel_reduce(_lib.ptr(points), _lib.ptr(colors), N, _lib.ptr(scratch), int(nb[0]),
+            _lib.check(lib.nslam_point_cloud_voxel_reduce(_lib.ptr(points), _lib.ptr(colors), N, _lib.ptr(scratch), scratch.numel(),
                                                           V, _lib.ptr(out_p), _lib.ptr(out_c), _lib.ptr(out_n),
                                                           _lib.stream_ptr()), "point_cloud_voxel_reduce")
         return out_p, out_c, out_n

@@ -56,7 +56,8 @@ class NgpModel(ctypes.Structure):
                [("aabb_scale", ctypes.c_float), ("cascades", ctypes.c_int), ("cone", ctypes.c_float),
                 ("near_distance", ctypes.c_float),
                 ("scale", ctypes.c_float * 16), ("res", ctypes.c_int * 16), ("size", ctypes.c_uint * 16),
-                ("offset", ctypes.c_uint * 16), ("dense", ctypes.c_int * 16), ("n_grid", ctypes.c_uint)]
+                ("offset", ctypes.c_uint * 16), ("dense", ctypes.c_int * 16), ("n_grid", ctypes.c_uint),
+                ("grid_grad_fx", ctypes.c_void_p), ("mlp_grad_part", ctypes.c_void_p), ("part_rows", ctypes.c_int)]
 
 
 class NgpImages(ctypes.Structure):
@@ -67,7 +68,7 @@ class NgpImages(ctypes.Structure):
 class NgpBatch(ctypes.Structure):
     _fields_ = [(n, ctypes.c_void_p) for n in ("rays", "coords", "tdist", "rgbsigma", "dout", "counters", "loss")] + \
                [(n, ctypes.c_int) for n in ("max_rays", "max_samples")] + \
-               [(n, ctypes.c_void_p) for n in ("enc", "denc")]
+               [(n, ctypes.c_void_p) for n in ("enc", "denc", "loss_fx")]
 
 
 def level_table(aabb_scale):
@@ -138,9 +139,11 @@ class _MeshKernels:
     def colors(self, tb, mesh, srgb):
         """mesh.vertex_colors <- the network's radiance at the vertices, seen from outside"""
         v, n = mesh.vertices, mesh.vertex_normals
+        nv = int(v.shape[0])
+        scratch = torch.empty(44 * min(nv, 1 << 18), dtype=torch.uint8, device=tb.device)
         _lib.check(_lib.load().nslam_ngp_mesh_colors(ctypes.byref(tb.model), _lib.ptr(tb.packed), _lib.ptr(v), _lib.ptr(n),
-                                                     int(v.shape[0]), int(bool(srgb)), _lib.ptr(mesh.vertex_colors),
-                                                     tb.num_sms, _lib.stream_ptr()), "ngp_mesh_colors")
+                                                     nv, int(bool(srgb)), _lib.ptr(mesh.vertex_colors), _lib.ptr(scratch),
+                                                     scratch.numel(), tb.num_sms, _lib.stream_ptr()), "ngp_mesh_colors")
 
 
 class _Training:
@@ -277,10 +280,15 @@ class Testbed:
         self.density = -torch.ones(ncell, **f)
         self.bits = torch.zeros(ncell // 8, dtype=torch.uint8, device=dev)
         self.stats = torch.zeros(2, **f)
+        # gradient scratch of the tensor-core backward: the fixed-point hash-grid accumulator and one row of weight-gradient
+        # partials per CTA, as many rows as the device has SMs so that every NSLAM_NERF_SMS budget fits
+        self.grid_grad_fx = torch.zeros(total * 2, dtype=torch.int64, device=dev)
+        self.mlp_grad_part = torch.zeros(torch.cuda.get_device_properties(dev).multi_processor_count, W_TOTAL, **f)
         m = NgpModel()
         for name in ("grid_half", "grid_master", "grid_grad", "grid_m", "grid_v", "mlp", "mlp_grad", "mlp_m",
-                     "mlp_v", "density", "bits", "stats"):
+                     "mlp_v", "density", "bits", "stats", "grid_grad_fx", "mlp_grad_part"):
             setattr(m, name, getattr(self, name).data_ptr())
+        m.part_rows = self.mlp_grad_part.shape[0]
         m.aabb_scale = self.aabb_scale; m.cascades = self.cascades
         m.cone = 1.0 / 256.0 if aabb_scale > 1 else 0.0
         m.near_distance = self.nerf.training.near_distance
@@ -296,6 +304,7 @@ class Testbed:
         self.cams_base = torch.zeros(self.n_images, 18, **f)
         self.cam_state = torch.zeros(3, self.n_images, 6, **f)
         self.cam_grad = torch.zeros(self.n_images, 6, **f)
+        self.cam_grad_fx = torch.zeros(self.n_images, 6, dtype=torch.int64, device=dev)
         self.cam_steps = torch.zeros(self.n_images, dtype=torch.int32, device=dev)
         self._lv = {k: np.ascontiguousarray(np.asarray([r[i] for r in rows], dt)) for i, (k, dt) in
                     enumerate((("scale", np.float32), ("res", np.int32), ("size", np.uint32), ("offset", np.uint32), ("dense", np.int32)))}
@@ -307,7 +316,8 @@ class Testbed:
                           dout=torch.zeros(self.max_samples, 4, **f),
                           counters=torch.zeros(4, dtype=torch.int32, device=dev), loss=torch.zeros(1, **f),
                           enc=torch.zeros(self.max_samples, 32, dtype=torch.float16, device=dev),
-                          denc=torch.zeros(self.max_samples, 32, dtype=torch.float16, device=dev))
+                          denc=torch.zeros(self.max_samples, 32, dtype=torch.float16, device=dev),
+                          loss_fx=torch.zeros(1, dtype=torch.int64, device=dev))
         for k, v in self._bufs.items():
             setattr(b, k, v.data_ptr())
         b.max_rays, b.max_samples = self.max_rays, self.max_samples
@@ -412,8 +422,8 @@ class Testbed:
                                               lv["size"].ctypes.data, lv["offset"].ctypes.data, lv["dense"].ctypes.data,
                                               float(self.aabb_scale), _lib.ptr(self._bufs["rays"]), int(self.rays_per_batch),
                                               _lib.ptr(self._bufs["coords"]), _lib.ptr(self._bufs["tdist"]), _lib.ptr(self._bufs["denc"]),
-                                              float(self.loss_scale), _lib.ptr(self.cam_grad), int(self.cam_grad.shape[0]),
-                                              _lib.stream_ptr()), "ngp_cam_grad")
+                                              float(self.loss_scale), _lib.ptr(self.cam_grad), _lib.ptr(self.cam_grad_fx),
+                                              int(self.cam_grad.shape[0]), _lib.stream_ptr()), "ngp_cam_grad")
         if self.grad_hook is not None:
             self.grad_hook(self)
         if refine:

@@ -43,10 +43,8 @@ class _CudaKernels:
         H, W = f["idepth"].shape
         n = 4 * H * W
         if vol._act is None or vol._act[0] != (H, W):
-            nbytes = np.zeros(1, np.int64)
-            _lib.check(lib.nslam_tsdf_blocks_scratch(H, W, nbytes.ctypes.data), "tsdf_blocks_scratch")
             dev = vol.device
-            vol._act = ((H, W), torch.empty(int(nbytes[0]), dtype=torch.uint8, device=dev),
+            vol._act = ((H, W), torch.empty(_lib.query_size("nslam_tsdf_blocks_scratch", H, W), dtype=torch.uint8, device=dev),
                         torch.empty(n, dtype=torch.int32, device=dev), torch.empty(n, dtype=torch.int64, device=dev),
                         torch.empty(2, dtype=torch.int32, device=dev), torch.empty(2, dtype=torch.int32).pin_memory())
         _, scratch, touched, new_keys, counts_dev, counts_host = vol._act
@@ -170,7 +168,7 @@ class VoxelBlockVolume:
         head = (_lib.ptr(self.tsdf), _lib.ptr(self.weight))
         blocks = (_lib.ptr(nbr), _lib.ptr(self._coords), self.n_blocks)
         mw = float(min_weight)
-        return marching_cubes("tsdf_blocks_mesh", partial(lib.nslam_tsdf_blocks_mesh_plan, self.n_blocks),
+        return marching_cubes("tsdf_blocks_mesh", (self.n_blocks,),
                               partial(lib.nslam_tsdf_blocks_mesh_count, *head, *blocks, mw),
                               partial(lib.nslam_tsdf_blocks_mesh_emit, *head, _lib.ptr(self.color), *blocks,
                                       float(self.voxel_size), mw), self.device)

@@ -57,14 +57,12 @@ class TsdfMesh:
         write_binary_ply(path, cols, self.triangles.detach().cpu().numpy())
 
 
-def marching_cubes(name, plan, count, emit, device):
-    """the host side of both marching-cubes read-outs: `plan`, `count` and `emit` are nslam_<name>_plan / _count / _emit
-    with the volume's leading arguments bound.  The count passes leave the vertex, triangle and active-voxel totals at the
+def marching_cubes(name, plan_args, count, emit, device):
+    """the host side of both marching-cubes read-outs: `plan_args` are the arguments of nslam_<name>_plan, `count` and
+    `emit` are nslam_<name>_count / _emit with the volume's leading arguments bound.  The count passes leave the vertex, triangle and active-voxel totals at the
     head of the scratch; their one host read sizes the outputs of the emit passes -> TsdfMesh of device tensors, or None
     when there is no triangle."""
-    n_scratch = np.zeros(1, np.int64)
-    _lib.check(plan(n_scratch.ctypes.data), name + "_plan")
-    scratch = torch.empty(int(n_scratch[0]), dtype=torch.int32, device=device)
+    scratch = torch.empty(_lib.query_size(f"nslam_{name}_plan", *plan_args), dtype=torch.int32, device=device)
     with _lib.fixed_stream():
         _lib.check(count(_lib.ptr(scratch), _lib.stream_ptr()), name + "_count")
         n_vert, n_tri, n_active = scratch[:3].tolist()
@@ -88,7 +86,7 @@ def mesh_dense(tsdf, weight, color, origin, voxel_size, min_weight):
     org = np.ascontiguousarray(np.asarray(origin, np.float32))
     mw = float(min_weight)
     return marching_cubes(
-        "tsdf_mesh", partial(lib.nslam_tsdf_mesh_plan, nx, ny, nz),
+        "tsdf_mesh", (nx, ny, nz),
         partial(lib.nslam_tsdf_mesh_count, _lib.ptr(tsdf), _lib.ptr(weight), nx, ny, nz, mw),
         partial(lib.nslam_tsdf_mesh_emit, _lib.ptr(tsdf), _lib.ptr(weight), _lib.ptr(color), nx, ny, nz, org.ctypes.data,
                 float(voxel_size), mw), tsdf.device)

@@ -25,8 +25,10 @@ int main(void) {
   SZ(nslam_update_ctx); OFF(nslam_update_ctx, ep); OFF(nslam_update_ctx, net); OFF(nslam_update_ctx, upmask);
   OFF(nslam_update_ctx, wp); OFF(nslam_update_ctx, bias); OFF(nslam_update_ctx, glo_w); OFF(nslam_update_ctx, e16);
   SZ(nslam_ngp_model); OFF(nslam_ngp_model, aabb_scale); OFF(nslam_ngp_model, scale); OFF(nslam_ngp_model, n_grid);
+  OFF(nslam_ngp_model, grid_grad_fx); OFF(nslam_ngp_model, mlp_grad_part); OFF(nslam_ngp_model, part_rows);
   SZ(nslam_ngp_images); OFF(nslam_ngp_images, n_active); OFF(nslam_ngp_images, W);
   SZ(nslam_ngp_batch); OFF(nslam_ngp_batch, max_rays); OFF(nslam_ngp_batch, enc); OFF(nslam_ngp_batch, denc);
+  OFF(nslam_ngp_batch, loss_fx);
   printf("enum NSLAM_W_COUNT %d\n", (int)NSLAM_W_COUNT);
   return 0;
 }

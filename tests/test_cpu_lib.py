@@ -49,3 +49,17 @@ def test_product_code_never_touches_the_oracle():
                 if pat.search(txt):
                     bad.append(os.path.join(root, f))
     assert not bad, bad
+
+
+def test_library_keeps_no_hidden_device_state():
+    """the caller owns all device memory and the library never synchronises: no allocation, free or synchronous memset
+    in csrc/, and the per-device dynamic shared-memory attribute is set only through ensure_dyn_smem"""
+    csrc = os.path.join(ROOT, "nerf_slam_b200", "csrc")
+    src = {f: open(os.path.join(csrc, f)).read() for f in sorted(os.listdir(csrc)) if f.endswith((".cu", ".cuh"))}
+    for f, txt in src.items():
+        assert not re.search(r"\bcuda(Malloc|Free)\w*\s*\(", txt), f
+        assert not re.search(r"\bcudaMemset(2D|3D)?\s*\(", txt), f
+        assert "static bool configured" not in txt, f
+    helper = re.search(r"cudaError_t ensure_dyn_smem\(.*?\n}\n", src["common.cuh"], flags=re.S)
+    assert helper and helper.group(0).count("cudaFuncSetAttribute(") == 1
+    assert sum(txt.count("cudaFuncSetAttribute") for txt in src.values()) == 1

@@ -222,8 +222,9 @@ def test_room_mesh_is_deterministic(room):
 def test_memory_at_512(room):
     """peak device memory added by a 512^3 read-out: 8 B per lattice point (field + weight), the marching cubes'
     scratch (4 + 3 ints per 256 points, 16 B per active voxel <= vertices + triangles) and outputs (36 B per vertex,
-    12 B per triangle), plus a 1 MiB margin (allocator rounding, count read-back).  The colour pass's chunk scratch is
-    library-owned (at most 11.5 MB, allocated once) and not counted here."""
+    12 B per triangle), plus a 1 MiB margin (allocator rounding, count read-back).  The colour pass's chunk scratch (44 B
+    per vertex of a chunk of at most 2^18, 11.5 MB) is allocated after the field and weight are freed, so the peak
+    does not include it."""
     tb = room.ngp
     torch.cuda.synchronize()
     base = torch.cuda.memory_allocated()

@@ -140,11 +140,12 @@ def test_loss_and_gradients_match_autograd(backend, R, per, tol):
     assert cos > (0.999999 if backend == "simt" else 0.9995), cos
 
 
-def test_camera_pose_gradients_match_autograd():
-    """optimize_extrinsics (fusion/nerf_fusion.py:99): nslam_ngp_cam_grad — dL/d(translation) and dL/d(rotation vector)
-    per camera from the batch's encoding gradients — against autograd through the oracle network with the sample
-    positions p = (o + dt_c) + t (d + w_c x d) (direction held fixed inside the spherical harmonics, as the published
-    scheme does).  Then one Adam step moves the effective camera against the gradient and an ingest resets it."""
+def test_camera_pose_gradients_through_caller_accumulator_match_autograd():
+    """optimize_extrinsics (fusion/nerf_fusion.py:99): nslam_ngp_cam_grad, through the caller-owned fixed-point accumulator
+    cam_grad_fx — dL/d(translation) and dL/d(rotation vector) per camera from the batch's encoding gradients — against
+    autograd through the oracle network with the sample positions p = (o + dt_c) + t (d + w_c x d) (direction held fixed
+    inside the spherical harmonics, as the published scheme does).  Then one Adam step moves the effective camera against
+    the gradient and an ingest resets it."""
     from nerf_slam_b200 import _lib
     tb = _testbed(seed=8)
     lib = _lib.load()
@@ -179,7 +180,8 @@ def test_camera_pose_gradients_match_autograd():
     _lib.check(lib.nslam_ngp_cam_grad(_lib.ptr(tb.grid_half), lv["scale"].ctypes.data, lv["res"].ctypes.data, lv["size"].ctypes.data,
                                       lv["offset"].ctypes.data, lv["dense"].ctypes.data, 4.0, _lib.ptr(tb._bufs["rays"]), R,
                                       _lib.ptr(tb._bufs["coords"]), _lib.ptr(tb._bufs["tdist"]), _lib.ptr(tb._bufs["denc"]), 1024.0,
-                                      _lib.ptr(tb.cam_grad), int(tb.cam_grad.shape[0]), _lib.stream_ptr()), "cam_grad")
+                                      _lib.ptr(tb.cam_grad), _lib.ptr(tb.cam_grad_fx), int(tb.cam_grad.shape[0]), _lib.stream_ptr()),
+               "cam_grad")
     torch.cuda.synchronize()
     # oracle
     P = _oracle_params(tb)
