@@ -116,6 +116,11 @@ _SIGNATURES = {
                            _P],
     "nslam_eval_visible": [_P, c_int, _P, c_int, _P, c_int, c_int, _P, c_float, c_float, c_float, _P, _P],
     "nslam_eval_reduce": [_P, c_int, c_float, c_float, _P, _P],
+    # triangle-mesh rendering (include/nslam_render.h)
+    "nslam_render_bvh_scratch": [c_int, c_int, _P],
+    "nslam_render_bvh_build": [_P, c_int, _P, c_int, c_int, _P, ctypes.c_longlong, _P, _P],
+    "nslam_render_views": [_P, ctypes.c_longlong, c_int, c_int, _P, _P, c_int, _P, c_int, c_int, c_float, c_float, c_int,
+                           c_int, _P, _P, _P, _P, _P],
     "nslam_ba_reduced_camera_matrix": [ctypes.POINTER(BAGraph), ctypes.POINTER(BABuffers), _P],
     "nslam_ba_tile_pixels": [],
     "nslam_ba_solve": [_P, _P, c_int, c_int, _P, c_float, c_float, c_float, _P, _P, _P, _P, _P],

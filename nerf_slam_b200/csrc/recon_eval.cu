@@ -19,7 +19,7 @@
 // Nearest neighbour.  The distance of query q to reference r is sqrt(fp64 ((dx² + dy²) + dz²)) with d = q - r of the
 // fp32 coordinates in fp64, rounded to fp32 once.  The nearest reference is the one with the smallest fp64 squared
 // distance, ties to the smaller reference index; only references with squared distance < max_dist² (fp64) count
-// (cKDTree's distance_upper_bound); none -> +inf and -1.  The BVH (Karras 2012): 63-bit Morton keys of the points
+// (cKDTree's distance_upper_bound); none -> +inf and -1.  The BVH (Karras 2012; lbvh.cuh): 63-bit Morton keys of the points
 // quantised to 2^21 cells per axis of their bounding box, CUB radix SortPairs of (key, index) (stable, so the index
 // breaks ties), leaf buckets of `leaf_size` consecutive sorted points, L - 1 internal nodes from the buckets' first
 // keys (equal keys split by bucket index), boxes bottom-up (min / max: exact, whatever order threads arrive in).
@@ -40,6 +40,7 @@
 // Scratch: sampling 16 B per triangle + CUB's scan storage; the BVH about 110 B per reference point (keys, indices, the
 // sorted points, 2 L - 1 node boxes, links, CUB's sort storage); the queries 24 B per query + CUB's sort storage.
 #include "nslam_eval.h"
+#include "lbvh.cuh"
 #include "tsdf_rules.cuh"
 
 #include <climits>
@@ -143,76 +144,7 @@ static size_t surface_scratch(int nt, void* base, SurfaceScratch* s) {
 }
 
 // ----------------------------------------------------------------------------------------------------------------- BVH
-constexpr int kMortonBits = 21;
 constexpr int kStack = 96;      // > the deepest tree: 63 key bits + 31 bits of bucket index among equal keys
-
-// order-preserving map of fp32 to u32, so that integer atomics give the exact min / max
-__device__ __forceinline__ unsigned ev_ord(float f) {
-  const unsigned b = __float_as_uint(f);
-  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float ev_unord(unsigned o) {
-  return __uint_as_float((o & 0x80000000u) ? (o & 0x7fffffffu) : ~o);
-}
-
-__device__ __forceinline__ unsigned long long ev_spread(unsigned v) {
-  unsigned long long x = v & 0x1fffffu;
-  x = (x | x << 32) & 0x1f00000000ffffull;
-  x = (x | x << 16) & 0x1f0000ff0000ffull;
-  x = (x | x << 8) & 0x100f00f00f00f00full;
-  x = (x | x << 4) & 0x10c30c30c30c30c3ull;
-  x = (x | x << 2) & 0x1249249249249249ull;
-  return x;
-}
-
-// Morton key of p in the box bounds (ordered lo[3], hi[3]); outside points clamp to the nearest cell
-__device__ __forceinline__ unsigned long long ev_morton(float x, float y, float z, const unsigned* bounds) {
-  const float p[3] = {x, y, z};
-  unsigned q[3];
-#pragma unroll
-  for (int c = 0; c < 3; c++) {
-    const float lo = ev_unord(bounds[c]), hi = ev_unord(bounds[3 + c]);
-    const float ext = hi - lo;
-    float f = ext > 0.f ? (p[c] - lo) / ext * (float)(1 << kMortonBits) : 0.f;
-    f = fminf(fmaxf(f, 0.f), (float)((1 << kMortonBits) - 1));   // NaN -> 0
-    q[c] = (unsigned)f;
-  }
-  return ev_spread(q[0]) << 2 | ev_spread(q[1]) << 1 | ev_spread(q[2]);
-}
-
-__global__ void __launch_bounds__(256) ev_bounds_kernel(const float* P, int n, unsigned* bounds) {
-  unsigned lo[3] = {0xffffffffu, 0xffffffffu, 0xffffffffu}, hi[3] = {0u, 0u, 0u};
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-#pragma unroll
-    for (int c = 0; c < 3; c++) {
-      const unsigned o = ev_ord(P[3 * (size_t)i + c]);
-      lo[c] = min(lo[c], o);
-      hi[c] = max(hi[c], o);
-    }
-  }
-#pragma unroll
-  for (int c = 0; c < 3; c++) {
-    for (int m = 16; m; m >>= 1) {
-      lo[c] = min(lo[c], __shfl_xor_sync(0xffffffffu, lo[c], m));
-      hi[c] = max(hi[c], __shfl_xor_sync(0xffffffffu, hi[c], m));
-    }
-  }
-  if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-    for (int c = 0; c < 3; c++) {
-      atomicMin(bounds + c, lo[c]);
-      atomicMax(bounds + 3 + c, hi[c]);
-    }
-  }
-}
-
-__global__ void __launch_bounds__(256) ev_keys_kernel(const float* P, int n, const unsigned* bounds, unsigned long long* keys,
-                                                      int* index) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  keys[i] = ev_morton(P[3 * (size_t)i], P[3 * (size_t)i + 1], P[3 * (size_t)i + 2], bounds);
-  index[i] = i;
-}
 
 __global__ void __launch_bounds__(256) ev_gather_kernel(const float* P, const int* order, int n, float4* pts) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -221,75 +153,19 @@ __global__ void __launch_bounds__(256) ev_gather_kernel(const float* P, const in
   pts[i] = make_float4(P[3 * (size_t)j], P[3 * (size_t)j + 1], P[3 * (size_t)j + 2], __int_as_float(j));
 }
 
-// common-prefix length of buckets i and j (keys = the sorted keys, bucket b starts at sorted position b * B); -1 when
-// j is outside [0, L)
-__device__ __forceinline__ int ev_delta(const unsigned long long* keys, int B, long long L, long long i, long long j) {
-  if (j < 0 || j >= L) return -1;
-  const unsigned long long ki = keys[i * B], kj = keys[j * B];
-  return ki == kj ? 64 + __clz((int)(i ^ j)) : __clzll((long long)(ki ^ kj));
-}
-
-// Karras 2012: node ids 0 .. L-2 internal, L-1 .. 2L-2 the leaves (leaf l = L-1+l); the root is node 0
-__global__ void __launch_bounds__(256) ev_internal_kernel(const unsigned long long* keys, int B, int L, int2* child,
-                                                          int* parent) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= L - 1) return;
-  const int d = ev_delta(keys, B, L, i, i + 1) - ev_delta(keys, B, L, i, i - 1) >= 0 ? 1 : -1;
-  const int dmin = ev_delta(keys, B, L, i, i - d);
-  long long lmax = 2;
-  while (ev_delta(keys, B, L, i, i + lmax * d) > dmin) lmax *= 2;
-  long long l = 0;
-  for (long long t = lmax / 2; t >= 1; t /= 2)
-    if (ev_delta(keys, B, L, i, i + (l + t) * d) > dmin) l += t;
-  const long long j = i + l * d;
-  const int dnode = ev_delta(keys, B, L, i, j);
-  long long s = 0, t = l;
-  do {
-    t = (t + 1) >> 1;
-    if (ev_delta(keys, B, L, i, i + (s + t) * d) > dnode) s += t;
-  } while (t > 1);
-  const int gamma = (int)(i + s * d + min(d, 0));
-  const int lo = (int)min((long long)i, j), hi = (int)max((long long)i, j);
-  const int left = lo == gamma ? L - 1 + gamma : gamma;
-  const int right = hi == gamma + 1 ? L - 1 + gamma + 1 : gamma + 1;
-  child[i] = make_int2(left, right);
-  parent[left] = i;
-  parent[right] = i;
-  if (i == 0) parent[0] = -1;
-}
-
-// leaf boxes, then up the tree: the second child to arrive at a node writes its box
-__global__ void __launch_bounds__(256) ev_boxes_kernel(const float4* pts, int n, int B, int L, const int2* child,
-                                                       const int* parent, int* flags, float* box) {
-  const int l = blockIdx.x * blockDim.x + threadIdx.x;
-  if (l >= L) return;
-  float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
-  const int s = l * B, e = min(n, s + B);
-  for (int j = s; j < e; j++) {
-    const float4 p = pts[j];
-    lo[0] = fminf(lo[0], p.x); lo[1] = fminf(lo[1], p.y); lo[2] = fminf(lo[2], p.z);
-    hi[0] = fmaxf(hi[0], p.x); hi[1] = fmaxf(hi[1], p.y); hi[2] = fmaxf(hi[2], p.z);
-  }
-  int node = L - 1 + l;
-  float* b = box + 6 * (size_t)node;
-  for (int c = 0; c < 3; c++) { b[c] = lo[c]; b[3 + c] = hi[c]; }
-  __threadfence();
-  node = parent[node];
-  while (node >= 0) {
-    if (atomicAdd(flags + node, 1) == 0) return;           // the sibling's box is not written yet: it goes on
-    __threadfence();
-    const int2 ch = child[node];
-    const float* b0 = box + 6 * (size_t)ch.x;
-    const float* b1 = box + 6 * (size_t)ch.y;
-    float* bn = box + 6 * (size_t)node;
-    for (int c = 0; c < 3; c++) {
-      bn[c] = fminf(__ldcg(b0 + c), __ldcg(b1 + c));
-      bn[3 + c] = fmaxf(__ldcg(b0 + 3 + c), __ldcg(b1 + 3 + c));
+// the box of leaf bucket l: min / max of its sorted points
+struct PointLeaf {
+  const float4* pts;
+  int n, B;
+  __device__ void operator()(int l, float lo[3], float hi[3]) const {
+    const int s = l * B, e = min(n, s + B);
+    for (int j = s; j < e; j++) {
+      const float4 p = pts[j];
+      lo[0] = fminf(lo[0], p.x); lo[1] = fminf(lo[1], p.y); lo[2] = fminf(lo[2], p.z);
+      hi[0] = fmaxf(hi[0], p.x); hi[1] = fmaxf(hi[1], p.y); hi[2] = fmaxf(hi[2], p.z);
     }
-    __threadfence();
-    node = parent[node];
   }
-}
+};
 
 struct BvhLayout {
   unsigned* bounds;              // [6] ordered fp32: lo xyz, hi xyz
@@ -490,11 +366,6 @@ __global__ void __launch_bounds__(256) ev_reduce_kernel(const float* dist, int n
   }
 }
 
-static int ev_grid(int n, int threads, int cap) {
-  const long long b = ((long long)n + threads - 1) / threads;
-  return (int)(b < cap ? (b > 0 ? b : 1) : cap);
-}
-
 }  // namespace nslam
 
 extern "C" {
@@ -570,7 +441,8 @@ int nslam_eval_bvh_build(const float* ref, int n_ref, int leaf_size, void* bvh, 
   } else if ((e = cudaMemsetAsync(s.parent, 0xff, sizeof(int), st)) != cudaSuccess) {
     return (int)e;
   }
-  ev_boxes_kernel<<<(s.L + 255) / 256, 256, 0, st>>>(s.pts, n_ref, leaf_size, s.L, s.child, s.parent, s.flags, s.box);
+  ev_boxes_kernel<<<(s.L + 255) / 256, 256, 0, st>>>(PointLeaf{s.pts, n_ref, leaf_size}, s.L, s.child, s.parent, s.flags,
+                                                     s.box);
   NSLAM_CHECK_LAUNCH();
   return 0;
 }

@@ -10,6 +10,16 @@ clouds as they are; every nearest-neighbour distance is exact (a linear BVH, not
     m["accuracy"], m["completion"], m["f_score"]
     trajectory_error(estimated_cam_T_world, gt_cam_T_world, align="sim3")["rmse"]
 
+Ground truth given only as a mesh is culled for occlusion with depth rendered from it (mesh_render.MeshScene):
+
+    gt = MeshScene((gt_vertices, gt_triangles))
+    m = reconstruction_metrics(rec, gt_mesh, gt_mask=lambda p: visible(p, poses, intr, W, H,
+                                                                          depths=gt.render(poses, intr, W, H).depth))
+
+and the depth metric of dense neural SLAM compares rendered views of two meshes:
+
+    mesh_depth_l1(fusion.build_mesh(0.5), (gt_vertices, gt_triangles), poses, intr, W, H)["depth_l1"]
+
 Inputs: `TsdfMesh` (TsdfFusion / NerfFusion.build_mesh), `point_cloud.PointCloud`, a (vertices, triangles) pair or a
 [N,3] point tensor.  Tensors must be CUDA tensors (there is no CPU path); numpy arrays are uploaded to the current
 device.  `read_ply` and `trajectory_error` are host code."""
@@ -233,6 +243,56 @@ def reconstruction_metrics(reconstruction, ground_truth, threshold=0.05, n_sampl
             "accuracy_fixed": s_acc, "completion_fixed": s_comp}
 
 
+def mesh_depth_l1(reconstruction, ground_truth, cam_T_world, intrinsics, width, height, max_dist=1.0, near=0.0,
+                  far=math.inf):
+    """Depth L1 between rendered views of two meshes -> dict: both are rendered (mesh_render.MeshScene, back faces
+    included) at the views cam_T_world [n,7] (t, q_xyzw) with intrinsics fx, fy, cx, cy at width x height, and
+
+      depth_l1        mean over the pixels both meshes hit of min(|d_rec - d_gt|, max_dist), metres
+      gt_hits         pixels the ground truth hits;  both_hits: pixels both hit
+      missing         pixels only the ground truth hits;  extra: pixels only the reconstruction hits
+      depth_l1_fixed  the sum of min(|d_rec - d_gt|, max_dist) as a 64-bit integer of 2^-32 m (nslam_eval_reduce):
+                      the same bits in every run
+    Each side is a TsdfMesh / NeRF mesh, a (vertices, triangles) pair or a MeshScene built before.  |d_rec - d_gt| is
+    the fp32 difference of the fp32 depths.  Views go in chunks of at most 2^31 / max_dist pixels (the fixed-point
+    sum's bound).  One host read (the sums), plus one per mesh given as a mesh (its build's validity flags)."""
+    from .mesh_render import MeshScene
+    md = float(max_dist)
+    if not (math.isfinite(md) and md > 0):
+        raise ValueError(f"max_dist must be positive and finite, got {max_dist}")
+    rec = reconstruction if isinstance(reconstruction, MeshScene) else MeshScene(reconstruction)
+    gt = ground_truth if isinstance(ground_truth, MeshScene) else MeshScene(ground_truth)
+    if rec.device != gt.device:
+        raise ValueError("reconstruction and ground truth must be on one device")
+    poses = _cuda_tensor(cam_T_world, torch.float32, "cam_T_world")
+    if poses.dim() != 2 or poses.shape[1] != 7:
+        raise ValueError(f"cam_T_world must be [n,7] (t, q_xyzw), got {tuple(poses.shape)}")
+    W, H, n = int(width), int(height), int(poses.shape[0])
+    if W <= 0 or H <= 0 or n == 0:
+        raise ValueError(f"need at least one view of positive size, got {n} views of {W} x {H}")
+    per_chunk = min(INT32_MAX, int(math.ceil(2.0 ** 31 / md)) - 1) // (H * W)
+    if per_chunk < 1:
+        raise ValueError(f"one {W} x {H} view exceeds the fixed-point sum's 2^31 / max_dist pixels")
+    chunks = range(0, n, per_chunk)
+    sums = torch.empty(len(chunks), 3, dtype=torch.int64, device=rec.device)
+    counts = torch.zeros(4, dtype=torch.int64, device=rec.device)
+    with _lib.fixed_stream():
+        for c, k0 in enumerate(chunks):
+            p = poses[k0:k0 + per_chunk]
+            a = rec.render(p, intrinsics, W, H, near, far)
+            b = gt.render(p, intrinsics, W, H, near, far)
+            hit_rec, hit_gt = a.triangle >= 0, b.triangle >= 0
+            both = hit_rec & hit_gt
+            diff = torch.where(both, (a.depth - b.depth).abs(), torch.zeros((), device=rec.device)).reshape(-1)
+            _metric_sums(diff, md, md, sums[c])
+            counts += torch.stack([hit_gt.sum(), both.sum(), (hit_gt & ~hit_rec).sum(), (hit_rec & ~hit_gt).sum()])
+        total = torch.cat([sums[:, 0].sum().reshape(1), counts]).tolist()
+    s, gt_hits, both_hits, missing, extra = total
+    return {"depth_l1": s / FIXED_POINT / both_hits if both_hits else math.nan, "gt_hits": gt_hits,
+            "both_hits": both_hits, "missing": missing, "extra": extra, "pixels": n * H * W, "max_dist": md,
+            "depth_l1_fixed": s}
+
+
 # ---------------------------------------------------------------------------------------------------------------- PLY
 _PLY_DTYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "i2", "int16": "i2", "ushort": "u2",
                "uint16": "u2", "int": "i4", "int32": "i4", "uint": "u4", "uint32": "u4", "float": "f4", "float32": "f4",
@@ -316,18 +376,20 @@ def _triangles(faces):
     return np.concatenate(tris).astype(np.int32) if tris else np.zeros((0, 3), np.int32)
 
 
-def read_ply(path):
+def read_ply(path, return_colors=False):
     """vertices [V,3] float32 and triangles [T,3] int32 (None when the file has no face element) of a PLY file: binary
     little- or big-endian or ASCII, x / y / z vertex properties of any numeric type, faces as a `vertex_indices` (or
     `vertex_index`) list, polygons fan-triangulated.  What TsdfMesh.write_ply / PointCloud.write_ply write, and the usual
-    ground-truth meshes and scans.  Other elements and properties are skipped."""
+    ground-truth meshes and scans.  Other elements and properties are skipped.  With `return_colors`, also the vertex
+    colours [V,3] float32 in [0,1] from red / green / blue (integer types divided by their maximum, 255 for uchar;
+    floats as stored), None when the file has none."""
     with open(path, "rb") as f:
         data = f.read()
     fmt, elements, body = _ply_header(data)
     endian = {"binary_little_endian": "<", "binary_big_endian": ">"}.get(fmt)
     tokens = data[body:].split() if fmt == "ascii" else None
     pos = body if endian else 0
-    vertices = triangles = None
+    vertices = triangles = colors = None
     for name, count, props in elements:
         if endian:
             vals, pos = _ply_binary_element(data, pos, count, props, endian)
@@ -337,6 +399,9 @@ def read_ply(path):
             if not all(k in vals for k in "xyz"):
                 raise ValueError("the vertex element has no x, y, z")
             vertices = np.stack([np.asarray(vals[k], np.float32) for k in "xyz"], 1)
+            if all(k in vals for k in ("red", "green", "blue")):
+                types = {n: t for n, t, _ in props}
+                colors = np.stack([_unit_color(vals[k], types[k]) for k in ("red", "green", "blue")], 1)
         elif name == "face":
             key = "vertex_indices" if "vertex_indices" in vals else "vertex_index"
             if key not in vals:
@@ -344,7 +409,16 @@ def read_ply(path):
             triangles = _triangles(vals[key])
     if vertices is None:
         raise ValueError("the PLY file has no vertex element")
-    return vertices, triangles
+    return (vertices, triangles, colors) if return_colors else (vertices, triangles)
+
+
+def _unit_color(values, ply_type):
+    """a colour channel on [0,1]: integers over their type's maximum, floats as stored"""
+    dt = np.dtype(ply_type)
+    a = np.asarray(values, np.float64)
+    if dt.kind in "iu":
+        return (a / np.iinfo(dt).max).astype(np.float32)
+    return a.astype(np.float32)
 
 
 # ------------------------------------------------------------------------------------------------------ trajectory error
