@@ -121,6 +121,18 @@ _SIGNATURES = {
     "nslam_render_bvh_build": [_P, c_int, _P, c_int, c_int, _P, ctypes.c_longlong, _P, _P],
     "nslam_render_views": [_P, ctypes.c_longlong, c_int, c_int, _P, _P, c_int, _P, c_int, c_int, c_float, c_float, c_int,
                            c_int, _P, _P, _P, _P, _P],
+    # triangle-mesh operations (include/nslam_mesh.h)
+    "nslam_mesh_components_scratch": [c_int, c_int, _P],
+    "nslam_mesh_components": [_P, c_int, _P, c_int, _P, ctypes.c_longlong, _P, _P, _P, _P, _P],
+    "nslam_mesh_submesh_scratch": [c_int, c_int, _P],
+    "nslam_mesh_submesh_count": [_P, c_int, c_int, _P, _P, ctypes.c_longlong, _P, _P],
+    "nslam_mesh_submesh_emit": [_P, _P, _P, c_int, _P, c_int, _P, ctypes.c_longlong, _P, _P, _P, _P, _P],
+    "nslam_mesh_any_vertex": [_P, _P, c_int, c_int, _P, _P, _P, _P],
+    "nslam_mesh_vertex_normals_scratch": [c_int, c_int, _P],
+    "nslam_mesh_vertex_normals": [_P, c_int, _P, c_int, _P, ctypes.c_longlong, _P, _P, _P],
+    "nslam_mesh_cluster_scratch": [c_int, c_int, _P],
+    "nslam_mesh_cluster_count": [_P, c_int, _P, c_int, c_float, _P, ctypes.c_longlong, _P, _P],
+    "nslam_mesh_cluster_emit": [_P, _P, c_int, _P, c_int, _P, ctypes.c_longlong, _P, _P, _P, _P],
     "nslam_ba_reduced_camera_matrix": [ctypes.POINTER(BAGraph), ctypes.POINTER(BABuffers), _P],
     "nslam_ba_tile_pixels": [],
     "nslam_ba_solve": [_P, _P, c_int, c_int, _P, c_float, c_float, c_float, _P, _P, _P, _P, _P],

@@ -41,6 +41,7 @@
 // sorted points, 2 L - 1 node boxes, links, CUB's sort storage); the queries 24 B per query + CUB's sort storage.
 #include "nslam_eval.h"
 #include "lbvh.cuh"
+#include "mesh_rules.cuh"
 #include "tsdf_rules.cuh"
 
 #include <climits>
@@ -74,29 +75,10 @@ __global__ void __launch_bounds__(256) ev_area_kernel(const float* V, int nv, co
     atomicOr(flags, 1ull);
     return;
   }
-  double e1[3], e2[3];
-#pragma unroll
-  for (int c = 0; c < 3; c++) {
-    const double a = V[3 * (size_t)ia + c];
-    e1[c] = __dsub_rn((double)V[3 * (size_t)ib + c], a);
-    e2[c] = __dsub_rn((double)V[3 * (size_t)ic + c], a);
-  }
-  const double x0 = __dsub_rn(__dmul_rn(e1[1], e2[2]), __dmul_rn(e1[2], e2[1]));
-  const double x1 = __dsub_rn(__dmul_rn(e1[2], e2[0]), __dmul_rn(e1[0], e2[2]));
-  const double x2 = __dsub_rn(__dmul_rn(e1[0], e2[1]), __dmul_rn(e1[1], e2[0]));
-  const double area = __dmul_rn(0.5, __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(x0, x0), __dmul_rn(x1, x1)), __dmul_rn(x2, x2))));
-  if (!isfinite(area)) {
-    w[t] = 0;
-    atomicOr(flags, 2ull);
-    return;
-  }
-  const double s = __dmul_rn(area, 0x1p40);
-  if (s > (double)cap) {
-    w[t] = 0;
-    atomicOr(flags, 4ull);
-    return;
-  }
-  w[t] = __double2ull_rn(s);
+  unsigned long long wt;
+  const unsigned f = tri_area_weight(V, ia, ib, ic, cap, wt);
+  w[t] = wt;
+  if (f) atomicOr(flags, (unsigned long long)f);
 }
 
 __global__ void __launch_bounds__(256) ev_sample_kernel(const float* V, const int* T, const unsigned long long* cdf, int nt,

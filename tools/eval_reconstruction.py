@@ -3,14 +3,21 @@ one JSON line: accuracy, completion, chamfer_l1 (metres), precision, recall, f_s
 counts.  Either file may be a mesh (a PLY with faces: sampled uniformly by area) or a point cloud (used as it is).
 
     python tools/eval_reconstruction.py rec.ply gt.ply [--threshold 0.05] [--samples 200000] [--max_dist 1.0] [--seed 0]
-                                        [--views transforms.json]
+                                        [--views transforms.json] [--cull] [--min_component_area A]
 
 With --views, both meshes are also rendered at the frames of a NeRF-style transforms.json (poses and intrinsics parsed
 as datasets.NeRFDataset does) and the line gains `mesh_depth_l1` (evaluation.mesh_depth_l1 with the same max_dist).
 
+--cull (needs --views and a ground-truth mesh) scores only what the cameras saw: the ground-truth mesh is rendered at
+the views, the reconstruction mesh is culled with that depth (mesh_ops.cull, a face goes when none of its vertices is
+seen) and the ground-truth samples are masked with it (evaluation.visible).  --min_component_area then drops the
+reconstruction's connected components smaller than A m^2 (mesh_ops.remove_small_components).  Without these flags the
+reconstruction is scored as it is.
+
 Needs a CUDA device."""
 import argparse
 import json
+import math
 import os
 import sys
 
@@ -26,37 +33,84 @@ def main(argv=None):
     ap.add_argument("--max_dist", type=float, default=1.0, help="distances are clamped here in the means (m)")
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--views", default=None, help="transforms.json whose frames to render both meshes at")
+    ap.add_argument("--cull", action="store_true", help="score only what the --views cameras saw")
+    ap.add_argument("--min_component_area", type=float, default=None,
+                    help="drop the reconstruction's connected components smaller than this (m^2)")
     a = ap.parse_args(argv)
+    if a.cull and not a.views:
+        ap.error("--cull needs --views")
+    if a.min_component_area is not None and not (math.isfinite(a.min_component_area) and a.min_component_area >= 0):
+        ap.error(f"--min_component_area must be finite and >= 0, got {a.min_component_area}")
     from nerf_slam_b200.evaluation import read_ply, reconstruction_metrics
 
     def load(path):
         v, t = read_ply(path)
         return (v, t) if t is not None and len(t) else v
 
-    m = reconstruction_metrics(load(a.reconstruction), load(a.ground_truth), threshold=a.threshold,
-                               n_samples=a.samples, max_dist=a.max_dist, seed=a.seed)
+    rec, gt = load(a.reconstruction), load(a.ground_truth)
+    gt_mask = None
+    cleaned = a.cull or a.min_component_area is not None
+    if cleaned:
+        rec, gt_mask = clean_reconstruction(rec, gt, a)
+    m = reconstruction_metrics(rec, gt, threshold=a.threshold, n_samples=a.samples, max_dist=a.max_dist, seed=a.seed,
+                               gt_mask=gt_mask)
     out = {"reconstruction": a.reconstruction, "ground_truth": a.ground_truth, **m}
-    if a.views:
+    if a.views and not cleaned:
         out["mesh_depth_l1"] = depth_at_views(a.reconstruction, a.ground_truth, a.views, a.max_dist)
+    elif a.views:
+        from nerf_slam_b200.evaluation import mesh_depth_l1
+        if not isinstance(gt, tuple):
+            raise SystemExit(f"--views renders meshes: {a.ground_truth} has no faces")
+        poses, intr, W, H = dataset_views(a.views)
+        out["mesh_depth_l1"] = mesh_depth_l1(rec, gt, poses, intr, W, H, max_dist=a.max_dist)
     print(json.dumps(out))
 
 
-def depth_at_views(rec_path, gt_path, views, max_dist):
-    """evaluation.mesh_depth_l1 of two PLY meshes at the frames of a transforms.json"""
+def clean_reconstruction(rec, gt, a):
+    """-> (the reconstruction culled to the views by the ground truth's rendered depth and / or without its small
+    components, the ground-truth mask under --cull or None)"""
+    from nerf_slam_b200 import mesh_ops
+    from nerf_slam_b200.evaluation import visible
+    from nerf_slam_b200.mesh_render import MeshScene
+    if not isinstance(rec, tuple):
+        raise SystemExit(f"--cull and --min_component_area act on meshes: {a.reconstruction} has no faces")
+    gt_mask = None
+    if a.cull:
+        if not isinstance(gt, tuple):
+            raise SystemExit(f"--cull renders the ground truth: {a.ground_truth} has no faces")
+        poses, intr, W, H = dataset_views(a.views)
+        gt_depth = MeshScene(gt).render(poses, intr, W, H).depth
+        rec = mesh_ops.cull(rec, poses, intr, W, H, depths=gt_depth)
+        gt_mask = lambda p: visible(p, poses, intr, W, H, depths=gt_depth)  # noqa: E731
+    if rec is not None and a.min_component_area is not None:
+        rec = mesh_ops.remove_small_components(rec, a.min_component_area)
+    if rec is None:
+        raise SystemExit("no triangle of the reconstruction remains after cleaning")
+    return rec, gt_mask
+
+
+def dataset_views(views):
+    """-> cam_T_world [n,7] fp32, intrinsics fx fy cx cy, width, height of the frames of a transforms.json"""
     import numpy as np
     from nerf_slam_b200.datasets import NeRFDataset, dataset_args
-    from nerf_slam_b200.evaluation import mesh_depth_l1, read_ply
     from nerf_slam_b200.frontend import matrix_to_tq
     ds = NeRFDataset(dataset_args(os.path.dirname(os.path.abspath(views)) or "."))
     cam, res = ds.calib.camera_model, ds.calib.resolution
     poses = np.asarray([matrix_to_tq(np.asarray(w2c, np.float64)) for w2c in ds.w2c], np.float32)
+    return poses, cam.numpy(), res.width, res.height
+
+
+def depth_at_views(rec_path, gt_path, views, max_dist):
+    """evaluation.mesh_depth_l1 of two PLY meshes at the frames of a transforms.json"""
+    from nerf_slam_b200.evaluation import mesh_depth_l1, read_ply
+    poses, intr, W, H = dataset_views(views)
     meshes = []
     for path in (rec_path, gt_path):
         v, t = read_ply(path)
         if t is None or not len(t):
             raise SystemExit(f"--views renders meshes: {path} has no faces")
         meshes.append((v, t))
-    return mesh_depth_l1(meshes[0], meshes[1], poses, cam.numpy(), res.width, res.height, max_dist=max_dist)
+    return mesh_depth_l1(meshes[0], meshes[1], poses, intr, W, H, max_dist=max_dist)
 
 
 if __name__ == "__main__":
