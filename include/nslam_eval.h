@@ -56,6 +56,29 @@ int nslam_eval_visible(const float* points, int n_points, const float* cam_T_wor
  * n * max_dist < 2^31 (the fixed-point sum then fits in 63 bits). */
 int nslam_eval_reduce(const float* dist, int n, float max_dist, float threshold, long long* out, void* stream);
 
+/* ---- registration (nerf_slam_b200/csrc/registration.cu, rules at its head): ICP against the BVH above. ---- */
+
+/* points [n,3] fp32 -> out [n,3] fp32 under the similarity sim3 (a HOST array of 13 doubles: s, R [3x3 row-major], t):
+ * s (R p) + t in fp64, rounded once; direction != 0 writes R p only (normals).  out may not alias points. */
+int nslam_reg_transform(const float* points, int n, const double* sim3, int direction, float* out, void* stream);
+
+/* normals [n,3] fp32: the unit (b - a) x (c - a) of triangle tri[i] of the mesh (vertices [n_vert,3] fp32, triangles
+ * [n_tri,3] int32), e.g. the triangles nslam_eval_sample_surface returns.  flags [1] (DEVICE int64): 1 an index out of
+ * range, 2 a zero or non-finite normal; such samples get 0. */
+int nslam_reg_face_normals(const float* vertices, int n_vert, const int* triangles, int n_tri, const int* tri, int n,
+                           float* normals, long long* flags, void* stream);
+
+/* The Gauss-Newton sums of one ICP iteration -> sums [38] (DEVICE int64, integers of 2^-27): source [n,3] fp32 (the
+ * transformed points), idx [n] int64 (nslam_eval_nearest's, -1: no correspondence) into target [n_target,3] fp32 and,
+ * unless point_to_point, target_normals [n_target,3] fp32 (unit).  frame is a HOST array of 4 doubles, the centre c and
+ * half-diagonal L of the target's box (L > 0, finite); correspondences must lie within L.  with_scale adds the scale
+ * unknown.  Layout: H's upper triangle over (omega, tau, sigma) row by row [28], g [7], the squared-residual sum, the
+ * count, flags (1 a target index out of range, 2 a term not below 16).  num_sms bounds the grid (<= 0: every SM); the
+ * sums do not depend on it. */
+int nslam_reg_accumulate(const float* source, int n, const long long* idx, const float* target, const float* target_normals,
+                         int n_target, const double* frame, int point_to_point, int with_scale, int num_sms, long long* sums,
+                         void* stream);
+
 #ifdef __cplusplus
 }
 #endif

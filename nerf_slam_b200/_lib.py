@@ -116,6 +116,10 @@ _SIGNATURES = {
                            _P],
     "nslam_eval_visible": [_P, c_int, _P, c_int, _P, c_int, c_int, _P, c_float, c_float, c_float, _P, _P],
     "nslam_eval_reduce": [_P, c_int, c_float, c_float, _P, _P],
+    # registration (include/nslam_eval.h); the double arrays are HOST arrays
+    "nslam_reg_transform": [_P, c_int, ctypes.POINTER(ctypes.c_double), c_int, _P, _P],
+    "nslam_reg_face_normals": [_P, c_int, _P, c_int, _P, c_int, _P, _P, _P],
+    "nslam_reg_accumulate": [_P, c_int, _P, _P, _P, c_int, ctypes.POINTER(ctypes.c_double), c_int, c_int, c_int, _P, _P],
     # triangle-mesh rendering (include/nslam_render.h)
     "nslam_render_bvh_scratch": [c_int, c_int, _P],
     "nslam_render_bvh_build": [_P, c_int, _P, c_int, c_int, _P, ctypes.c_longlong, _P, _P],

@@ -33,6 +33,51 @@ def min_bytes(op, nv, nt, out_v=0, out_t=0, n_views=0):
             "simplify_vertex_clustering": 24 * nv + 12 * nt + mesh_out}[op]
 
 
+def room_meshes(res, dev):
+    """-> the trained NeRF room's mesh with its 12 views (cam_T_world [12,7], intrinsics, (W, H)) and the dense TSDF mesh
+    of 10 room views with its views (cam_T_world [10,7], intrinsics), both at res^3"""
+    import torch
+    from nerf_slam_b200.frontend import matrix_to_tq
+    from nerf_slam_b200.nerf_fusion import NerfFusion
+    from nerf_slam_b200.synthetic import SyntheticRoom
+    from nerf_slam_b200.tsdf_fusion import TsdfFusion
+    T = lambda x: torch.from_numpy(np.ascontiguousarray(x)).to(dev)  # noqa: E731
+
+    # the trained NeRF room (tests/test_gpu_nerf_mesh.py's fixture)
+    nroom = SyntheticRoom(160, 120, 12, seed=0, half_extent=(1.4, 1.0, 1.4), orbit_radius=0.3, step=0.25)
+    nf = NerfFusion("nerf", types.SimpleNamespace(buffer=12, eval=False, mask_type="ours"), dev)
+    nf.ngp.nerf.training.depth_supervision_lambda = 1.0
+    nf.gt_fit_convention = "metric"
+    pk = [nroom.packet(k) for k in range(12)]
+    nf.fuse({"data": {"k": np.arange(12), "poses": np.stack([p["poses"][0] for p in pk]),
+                      "images": np.stack([p["images"][0] for p in pk]), "depths": np.stack([p["depths"][0] for p in pk]),
+                      "calibs": pk[0]["calibs"]}})
+    for _ in range(300):
+        nf.fit_volume_once()
+    nerf_mesh = nf.ngp.marching_cubes(res, None, 10.0)
+    nerf_poses = T(np.asarray([matrix_to_tq(np.asarray(nroom.render(k)[2], np.float64)) for k in range(12)], np.float32))
+    nerf_intr, nerf_wh = nroom.calib.camera_model.numpy().astype(np.float32), (nroom.W, nroom.H)
+    del nf
+    torch.cuda.empty_cache()
+
+    # the dense TSDF of 10 room views
+    room = SyntheticRoom(W, H, 200, seed=0)
+    intr = room.calib.camera_model.numpy().astype(np.float32)
+    ks = list(range(0, 200, 20))
+    poses = T(np.asarray([matrix_to_tq(np.asarray(room.render(k)[2], np.float64)) for k in ks], np.float32))
+    fus = TsdfFusion("tsdf", types.SimpleNamespace(eval=False, tsdf_volume="dense", tsdf_resolution=res), dev)
+    fus.voxel_size = 8.0 / res
+    fus.initialize()
+    depths = np.stack([room.render(k)[1][..., 0].astype(np.float32) * np.float32(room.calib.depth_scale) for k in ks])
+    images = np.stack([room.render(k)[0][..., :3].transpose(2, 0, 1) for k in ks])
+    fus.build_volume({"cam0_poses": poses, "cam0_idepths_up": T(1.0 / depths), "cam0_depths_cov_up": None,
+                      "cam0_images": T(images)}, intr, None)
+    tsdf_mesh = fus.build_mesh(0.5)
+    fus.volume = None
+    torch.cuda.empty_cache()
+    return nerf_mesh, nerf_poses, nerf_intr, nerf_wh, tsdf_mesh, poses, intr
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
@@ -40,11 +85,7 @@ def main():
     a = ap.parse_args()
     import torch
     from nerf_slam_b200 import _lib, mesh_ops
-    from nerf_slam_b200.frontend import matrix_to_tq
     from nerf_slam_b200.mesh_render import MeshScene
-    from nerf_slam_b200.nerf_fusion import NerfFusion
-    from nerf_slam_b200.synthetic import SyntheticRoom
-    from nerf_slam_b200.tsdf_fusion import TsdfFusion
     _lib.load()                                            # raises NslamUnavailable without CUDA: no fallback
     dev = "cuda:0"
     name, power = gpu_card()
@@ -63,40 +104,7 @@ def main():
             ts.append(e0.elapsed_time(e1))
         return out, float(np.median(ts))
 
-    T = lambda x: torch.from_numpy(np.ascontiguousarray(x)).to(dev)  # noqa: E731
-
-    # the trained NeRF room (tests/test_gpu_nerf_mesh.py's fixture)
-    nroom = SyntheticRoom(160, 120, 12, seed=0, half_extent=(1.4, 1.0, 1.4), orbit_radius=0.3, step=0.25)
-    nf = NerfFusion("nerf", types.SimpleNamespace(buffer=12, eval=False, mask_type="ours"), dev)
-    nf.ngp.nerf.training.depth_supervision_lambda = 1.0
-    nf.gt_fit_convention = "metric"
-    pk = [nroom.packet(k) for k in range(12)]
-    nf.fuse({"data": {"k": np.arange(12), "poses": np.stack([p["poses"][0] for p in pk]),
-                      "images": np.stack([p["images"][0] for p in pk]), "depths": np.stack([p["depths"][0] for p in pk]),
-                      "calibs": pk[0]["calibs"]}})
-    for _ in range(300):
-        nf.fit_volume_once()
-    nerf_mesh = nf.ngp.marching_cubes(a.res, None, 10.0)
-    nerf_poses = T(np.asarray([matrix_to_tq(np.asarray(nroom.render(k)[2], np.float64)) for k in range(12)], np.float32))
-    nerf_intr, nerf_wh = nroom.calib.camera_model.numpy().astype(np.float32), (nroom.W, nroom.H)
-    del nf
-    torch.cuda.empty_cache()
-
-    # the dense TSDF of 10 room views
-    room = SyntheticRoom(W, H, 200, seed=0)
-    intr = room.calib.camera_model.numpy().astype(np.float32)
-    ks = list(range(0, 200, 20))
-    poses = T(np.asarray([matrix_to_tq(np.asarray(room.render(k)[2], np.float64)) for k in ks], np.float32))
-    fus = TsdfFusion("tsdf", types.SimpleNamespace(eval=False, tsdf_volume="dense", tsdf_resolution=a.res), dev)
-    fus.voxel_size = 8.0 / a.res
-    fus.initialize()
-    depths = np.stack([room.render(k)[1][..., 0].astype(np.float32) * np.float32(room.calib.depth_scale) for k in ks])
-    images = np.stack([room.render(k)[0][..., :3].transpose(2, 0, 1) for k in ks])
-    fus.build_volume({"cam0_poses": poses, "cam0_idepths_up": T(1.0 / depths), "cam0_depths_cov_up": None,
-                      "cam0_images": T(images)}, intr, None)
-    tsdf_mesh = fus.build_mesh(0.5)
-    fus.volume = None
-    torch.cuda.empty_cache()
+    nerf_mesh, nerf_poses, nerf_intr, nerf_wh, tsdf_mesh, poses, intr = room_meshes(a.res, dev)
 
     res = {}
     for label, mesh, p, K, (w, h) in (("nerf_mesh", nerf_mesh, nerf_poses, nerf_intr, nerf_wh),
