@@ -17,6 +17,9 @@
 extern "C" {
 #endif
 
+/* blocks of the occupancy refresh's mean-density reduction: density_partials holds one (sum, count) pair per block */
+#define NSLAM_NGP_DENSITY_BLOCKS 592
+
 typedef struct nslam_ngp_model {
   void* grid_half;        /* __half2 [n_grid]   fp16 compute copy of the hash table            */
   float* grid_master;     /* [n_grid*2]         fp32 master                                    */
@@ -33,6 +36,7 @@ typedef struct nslam_ngp_model {
   long long* grid_grad_fx;  /* [n_grid*2]         fixed-point hash-grid gradient accumulator: zero on entry, zero on return */
   float* mlp_grad_part;     /* [part_rows,10240]  per-CTA weight-gradient partials of the tensor-core backward       */
   int part_rows;            /* rows of mlp_grad_part: nslam_ngp_backward_tc needs num_sms <= part_rows             */
+  float* density_partials;  /* [2*NSLAM_NGP_DENSITY_BLOCKS] per-block (sum, count) of nslam_ngp_update_density_grid's mean */
 } nslam_ngp_model;
 
 typedef struct nslam_ngp_images {

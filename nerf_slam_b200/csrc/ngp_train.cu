@@ -756,10 +756,11 @@ __global__ void density_mark_kernel(const Camera* __restrict__ cams, const int* 
 }
 
 // mean of the non-negative densities -> stats[0] = sum, stats[1] = count.  Fixed summation order (no atomics):
-// each block writes its partial, density_mean_final_kernel adds the partials in block order.
-constexpr int DM_BLOCKS = 592;
-__device__ float g_density_partials[2 * DM_BLOCKS];
-__global__ void __launch_bounds__(256) density_mean_kernel(const float* __restrict__ density, size_t n) {
+// each block writes its partial to the caller's partials[2 * block + {0, 1}], density_mean_final_kernel adds the
+// partials in block order.
+constexpr int DM_BLOCKS = NSLAM_NGP_DENSITY_BLOCKS;
+__global__ void __launch_bounds__(256) density_mean_kernel(const float* __restrict__ density, size_t n,
+                                                            float* __restrict__ partials) {
   __shared__ float ws[2][8];
   float s = 0.f, c = 0.f;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
@@ -772,13 +773,13 @@ __global__ void __launch_bounds__(256) density_mean_kernel(const float* __restri
   if (threadIdx.x < 2) {
     float v = 0.f;
     for (int w = 0; w < 8; w++) v += ws[threadIdx.x][w];
-    g_density_partials[2 * blockIdx.x + threadIdx.x] = v;
+    partials[2 * blockIdx.x + threadIdx.x] = v;
   }
 }
-__global__ void density_mean_final_kernel(float* __restrict__ stats) {
+__global__ void density_mean_final_kernel(const float* __restrict__ partials, float* __restrict__ stats) {
   if (threadIdx.x < 2) {
     float v = 0.f;
-    for (int b = 0; b < DM_BLOCKS; b++) v += g_density_partials[2 * b + threadIdx.x];
+    for (int b = 0; b < DM_BLOCKS; b++) v += partials[2 * b + threadIdx.x];
     stats[threadIdx.x] = v;
   }
 }
@@ -1033,8 +1034,8 @@ int nslam_ngp_update_density_grid(const nslam_ngp_model* m, const nslam_ngp_imag
                                                                        make_scene(m), n_per_cascade, seed, decay, m->density);
     NSLAM_CHECK_LAUNCH();
   }
-  density_mean_kernel<<<DM_BLOCKS, 256, 0, st>>>(m->density, total);
-  density_mean_final_kernel<<<1, 32, 0, st>>>(m->stats);
+  density_mean_kernel<<<DM_BLOCKS, 256, 0, st>>>(m->density, total, m->density_partials);
+  density_mean_final_kernel<<<1, 32, 0, st>>>(m->density_partials, m->stats);
   NSLAM_CHECK_LAUNCH();
   density_bits_kernel<<<(unsigned)((total / 8 + 255) / 256), 256, 0, st>>>(m->density, total / 8, m->stats,
                                                                           min_thickness, m->bits);

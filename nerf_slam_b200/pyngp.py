@@ -30,6 +30,7 @@ from . import _lib
 N_LEVELS, LOG2_T, BASE_RES = 16, 19, 16
 W_TOTAL = 10240
 GRID = 128
+DENSITY_BLOCKS = 592          # NSLAM_NGP_DENSITY_BLOCKS (include/nslam_ngp.h)
 
 
 class TestbedMode:
@@ -57,7 +58,8 @@ class NgpModel(ctypes.Structure):
                 ("near_distance", ctypes.c_float),
                 ("scale", ctypes.c_float * 16), ("res", ctypes.c_int * 16), ("size", ctypes.c_uint * 16),
                 ("offset", ctypes.c_uint * 16), ("dense", ctypes.c_int * 16), ("n_grid", ctypes.c_uint),
-                ("grid_grad_fx", ctypes.c_void_p), ("mlp_grad_part", ctypes.c_void_p), ("part_rows", ctypes.c_int)]
+                ("grid_grad_fx", ctypes.c_void_p), ("mlp_grad_part", ctypes.c_void_p), ("part_rows", ctypes.c_int),
+                ("density_partials", ctypes.c_void_p)]
 
 
 class NgpImages(ctypes.Structure):
@@ -280,13 +282,14 @@ class Testbed:
         self.density = -torch.ones(ncell, **f)
         self.bits = torch.zeros(ncell // 8, dtype=torch.uint8, device=dev)
         self.stats = torch.zeros(2, **f)
+        self.density_partials = torch.zeros(2 * DENSITY_BLOCKS, **f)     # per-block partials of the refresh's mean density
         # gradient scratch of the tensor-core backward: the fixed-point hash-grid accumulator and one row of weight-gradient
         # partials per CTA, as many rows as the device has SMs so that every NSLAM_NERF_SMS budget fits
         self.grid_grad_fx = torch.zeros(total * 2, dtype=torch.int64, device=dev)
         self.mlp_grad_part = torch.zeros(torch.cuda.get_device_properties(dev).multi_processor_count, W_TOTAL, **f)
         m = NgpModel()
         for name in ("grid_half", "grid_master", "grid_grad", "grid_m", "grid_v", "mlp", "mlp_grad", "mlp_m",
-                     "mlp_v", "density", "bits", "stats", "grid_grad_fx", "mlp_grad_part"):
+                     "mlp_v", "density", "bits", "stats", "grid_grad_fx", "mlp_grad_part", "density_partials"):
             setattr(m, name, getattr(self, name).data_ptr())
         m.part_rows = self.mlp_grad_part.shape[0]
         m.aabb_scale = self.aabb_scale; m.cascades = self.cascades

@@ -26,6 +26,8 @@ int main(void) {
   OFF(nslam_update_ctx, wp); OFF(nslam_update_ctx, bias); OFF(nslam_update_ctx, glo_w); OFF(nslam_update_ctx, e16);
   SZ(nslam_ngp_model); OFF(nslam_ngp_model, aabb_scale); OFF(nslam_ngp_model, scale); OFF(nslam_ngp_model, n_grid);
   OFF(nslam_ngp_model, grid_grad_fx); OFF(nslam_ngp_model, mlp_grad_part); OFF(nslam_ngp_model, part_rows);
+  OFF(nslam_ngp_model, density_partials);
+  printf("define NSLAM_NGP_DENSITY_BLOCKS %d\n", (int)NSLAM_NGP_DENSITY_BLOCKS);
   SZ(nslam_ngp_images); OFF(nslam_ngp_images, n_active); OFF(nslam_ngp_images, W);
   SZ(nslam_ngp_batch); OFF(nslam_ngp_batch, max_rays); OFF(nslam_ngp_batch, enc); OFF(nslam_ngp_batch, denc);
   OFF(nslam_ngp_batch, loss_fx);
@@ -61,6 +63,7 @@ def test_ctypes_mirrors_match_c_structs(c_layout):
             st, field = name.split(".")
             assert getattr(mirrors[st], field).offset == val, (name, getattr(mirrors[st], field).offset, val)
     assert c_layout[("enum", "NSLAM_W_COUNT")] == _lib.N_UPDATE_WEIGHTS
+    assert c_layout[("define", "NSLAM_NGP_DENSITY_BLOCKS")] == pyngp.DENSITY_BLOCKS
     from nerf_slam_b200.conv import UpdateOperatorTC
     assert len(UpdateOperatorTC.W_ORDER) == _lib.N_UPDATE_WEIGHTS
 

@@ -51,15 +51,46 @@ def test_product_code_never_touches_the_oracle():
     assert not bad, bad
 
 
+def _mutable_device_globals(txt):
+    """namespace-scope `__device__` / `__managed__` variables that are not const: device memory no caller owns, shared
+    by every user of the library in the process (the `__constant__` tables of tsdf_mesh.cu are read-only and allowed)"""
+    code = re.sub(r"//[^\n]*|/\*.*?\*/", "", txt, flags=re.S)
+    found, blocks = [], []            # blocks: True for a namespace / extern "C" block (its contents stay at namespace scope)
+    for piece in re.split(r"(?<=[;{}])", code):
+        stmt = " ".join(piece.split())
+        if stmt.endswith("}"):                                       # the end of a block or of a braced initialiser row
+            if blocks:
+                blocks.pop()
+            continue
+        words = stmt.rstrip(";{").replace("(", " ( ").split()
+        if all(blocks) and ("__device__" in words or "__managed__" in words) and "(" not in words \
+                and not {"const", "constexpr", "__constant__"} & set(words):
+            found.append(stmt)
+        if stmt.endswith("{"):
+            blocks.append(bool(re.search(r"\bnamespace\b[\w\s]*\{$|extern \"C\" \{$", stmt)))
+    return found
+
+
+def test_mutable_device_global_scan_finds_what_it_should():
+    src = ("namespace ngp {\n__device__ float g_partials[2 * 592];\n__device__ __forceinline__ float f(float x) { return x; }\n"
+           "__constant__ int c_tab[4] = {1, 2, 3, 4};\n__device__ const float k_half = 0.5f;\nstatic __device__ int counter = 0;\n"
+           "__global__ void k(float* o) { __shared__ float s[32]; o[0] = s[0]; }\n}  // namespace ngp\n"
+           "extern \"C\" {\n__managed__ int m_flag;\n}\n// __device__ float in_a_comment;\n")
+    assert _mutable_device_globals(src) == ["__device__ float g_partials[2 * 592];", "static __device__ int counter = 0;",
+                                            "__managed__ int m_flag;"]
+
+
 def test_library_keeps_no_hidden_device_state():
     """the caller owns all device memory and the library never synchronises: no allocation, free or synchronous memset
-    in csrc/, and the per-device dynamic shared-memory attribute is set only through ensure_dyn_smem"""
+    in csrc/, no mutable namespace-scope device variable (two callers on two streams would race on it), and the
+    per-device dynamic shared-memory attribute is set only through ensure_dyn_smem"""
     csrc = os.path.join(ROOT, "nerf_slam_b200", "csrc")
     src = {f: open(os.path.join(csrc, f)).read() for f in sorted(os.listdir(csrc)) if f.endswith((".cu", ".cuh"))}
     for f, txt in src.items():
         assert not re.search(r"\bcuda(Malloc|Free)\w*\s*\(", txt), f
         assert not re.search(r"\bcudaMemset(2D|3D)?\s*\(", txt), f
         assert "static bool configured" not in txt, f
+        assert not _mutable_device_globals(txt), (f, _mutable_device_globals(txt))
     helper = re.search(r"cudaError_t ensure_dyn_smem\(.*?\n}\n", src["common.cuh"], flags=re.S)
     assert helper and helper.group(0).count("cudaFuncSetAttribute(") == 1
     assert sum(txt.count("cudaFuncSetAttribute") for txt in src.values()) == 1
